@@ -7,6 +7,29 @@ import oracle
 GL = oracle.GOLDILOCKS
 _ctx = None
 
+# Test primes for the run-time-modulus (Montgomery, R = 2^64) policy, which every (p, g) except Goldilocks with g = 7
+# takes: name → (p, g, 2-adicity).  Each g is a quadratic non-residue, so ω = g^((p-1)/n) has order exactly n for
+# every n = 2^k up to the 2-adicity.
+BABYBEAR = 2013265921          # 15·2^27 + 1
+PBIG = 0xFFFFFFFF70000001      # above 2^63 and not Goldilocks: the subtractive REDC at every size
+MONT_PRIMES = {
+    "babybear": (BABYBEAR, 31, 27),                         # p < 2^31, every size to 2^26
+    "koalabear": (2130706433, 3, 24),                       # 127·2^24 + 1
+    "p32": (4295294977, 5, 16),                             # 0x100050001: residues straddle the 32-bit word boundary
+    "p57": (4179340454199820289, 3, 57),                    # 29·2^57 + 1
+    "pbig": (PBIG, 3, 28),
+    "gl_g5": (GL, pow(7, 5, GL), 32),                       # Goldilocks through the Montgomery kernels: ω' = ω^5
+    "p2adic3": ((1 << 64) - 279, 5, 3),                     # above 2^63, partial radix-16 constant table, n ≤ 8
+}
+for _name, (_p, _g, _s) in MONT_PRIMES.items():
+    assert pow(_g, (_p - 1) // 2, _p) == _p - 1, _name
+    assert ((_p - 1) & -(_p - 1)).bit_length() - 1 == _s, _name
+
+
+def s64(v):
+    """A uint64 residue as the int64 torch stores it."""
+    return int(np.array([v], dtype=np.uint64).view(np.int64)[0])
+
 
 def ctx():
     global _ctx

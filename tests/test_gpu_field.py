@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import oracle
-from gpu_util import GL, ctx, dev, host
+from gpu_util import BABYBEAR, GL, PBIG, ctx, dev, host
 
 pytestmark = pytest.mark.gpu
 
@@ -65,7 +65,7 @@ def _edge(p):
     return [x % p for x in v]
 
 
-@pytest.mark.parametrize("p", [GL, 0xFFFFFFFFFFFFFFC5, 0x7FFFFFFFFFFFFFE7, 4179340454199820289, 127])
+@pytest.mark.parametrize("p", [GL, 0xFFFFFFFFFFFFFFC5, 0x7FFFFFFFFFFFFFE7, 4179340454199820289, 127, BABYBEAR, 4295294977, PBIG])
 def test_64bit_field_ops_vs_oracle(p):
     from ronkathon_b200 import ops
     c = ctx()

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import oracle
-from gpu_util import GL, ctx, dev, host, summary
+from gpu_util import GL, MONT_PRIMES, PBIG, BABYBEAR, ctx, dev, host, s64, summary
 
 pytestmark = pytest.mark.gpu
 
@@ -77,20 +77,195 @@ def test_goldilocks_two_pass_sizes(log_n, batch):
     assert np.array_equal(gpu_ntt(X, log_n, batch, inverse=True), a)
 
 
+def _montgomery_cases():
+    sizes = {"babybear": range(1, 27), "pbig": range(1, 27), "koalabear": (1, 5, 9, 12, 13, 14, 15, 18, 21, 24),
+             "p32": range(1, 17), "p57": (1, 9, 13, 14, 15, 17, 20, 23, 26),
+             "gl_g5": (1, 2, 10, 13, 14, 15, 16, 20, 24, 25, 26), "p2adic3": (1, 2, 3)}
+    cases = [(name, lg, 1) for name in MONT_PRIMES for lg in sizes[name]]
+    return cases + [(name, lg, b) for name in ("babybear", "pbig") for lg, b in ((12, 64), (16, 3), (18, 17))]
+
+
+@pytest.mark.parametrize("name,log_n,batch", _montgomery_cases())
+def test_montgomery_transform_every_size(name, log_n, batch):
+    """Every (p, g) except Goldilocks with g = 7 runs on the run-time-modulus Montgomery kernels: the single-tile kernel up
+    to 2^13, the two-pass tile kernel from 2^14 to 2^26.  Single transforms shrink the tiles until the grid fills the GPU
+    (2^20: pass-1 tiles of 2^12 points, 128 threads; pass-2 tiles of 2^11, 128 threads); from 2^22 up the preferred
+    2^14-point pass-1 tile (512 threads) and 2^13-point pass-2 tile (256 threads) run.  The batches reach the same
+    preferred tiles at 17 × 2^18, 2^12-point single tiles (128 threads) at 64 × 2^12, and shrunken tiles at 3 × 2^16.
+    Forward against the oracle (bit for bit up to 2^22 words, else X[k] = a(ω^k) by Horner at sampled k), Goldilocks with
+    g = 7^5 against the g = 7 transform permuted by k → 5k mod n at full length, the fused point-wise multiply and the
+    inverse round trip.  The first two inputs are p - 1 and p - 2."""
+    _check_montgomery_transform(name, log_n, batch)
+
+
 def test_generic_montgomery_path_on_goldilocks_and_other_64bit_primes():
-    """A different generator sends Goldilocks through the run-time-modulus Montgomery kernels —
-    the path p = 101 uses — and must agree with the oracle; so must another NTT-friendly prime."""
-    g5 = oracle.pow_(GL, 7, 5)
-    for log_n in (10, 16):
-        a = oracle.splitmix(GL, 5, 1 << log_n)
-        assert np.array_equal(gpu_ntt(a, log_n, g=g5), oracle.ntt_fast(GL, a, g=g5))
-    p2 = 4179340454199820289  # 29·2^57 + 1
-    g2 = 3
-    for log_n in (9, 13, 17):
-        a = oracle.splitmix(p2, 6, 1 << log_n)
-        X = gpu_ntt(a, log_n, p=p2, g=g2)
-        assert np.array_equal(X, oracle.ntt_fast(p2, a, g=g2))
-        assert np.array_equal(gpu_ntt(X, log_n, inverse=True, p=p2, g=g2), a)
+    """A different generator sends Goldilocks through the run-time-modulus Montgomery kernels — the path p = 101
+    uses — and must agree with the oracle; so must another NTT-friendly prime.  The original cases (Goldilocks with
+    g = 7^5 at 2^10 and 2^16, 29·2^57 + 1 at 2^9, 2^13 and 2^17) with the checks of the every-size test above."""
+    for name, log_n in (("gl_g5", 10), ("gl_g5", 16), ("p57", 9), ("p57", 13), ("p57", 17)):
+        _check_montgomery_transform(name, log_n, 1)
+
+
+def _check_montgomery_transform(name, log_n, batch):
+    from ronkathon_b200 import ops
+    c = ctx()
+    p, g, _ = MONT_PRIMES[name]
+    n = 1 << log_n
+    a = host(ops.splitmix_fill(c, n * batch, 800 + log_n, p)).copy()
+    a[0], a[1] = p - 1, p - 2
+    m = ops.splitmix_fill(c, n * batch, 900 + log_n, p)
+    x = dev(a)
+    ops.ntt_(c, x, log_n, batch, False, p, g)
+    X = host(x)
+    if n * batch <= 1 << 22:
+        members = range(batch)
+    elif n <= 1 << 22:
+        members = sorted({0, batch // 2, batch - 1})
+    else:
+        members = []
+        w = oracle.root_of_unity(p, n, g)
+        for k in sorted({0, 1, n // 2 + 3, (n // 3) | 1, n - 1}):
+            assert int(X[k]) == oracle.poly_eval_horner(p, a[:n], oracle.pow_(p, w, k)), (name, log_n, k)
+    for b in members:
+        assert np.array_equal(X[b * n:(b + 1) * n], oracle.ntt_fast(p, a[b * n:(b + 1) * n], g=g)), (name, log_n, b)
+    if name == "gl_g5":
+        X7 = gpu_ntt(a, log_n, batch)
+        perm = (np.arange(n, dtype=np.uint64) * np.uint64(5)) % np.uint64(n)
+        assert np.array_equal(X.reshape(batch, n), X7.reshape(batch, n)[:, perm])
+        del X7, perm
+    y = dev(a)
+    ops.ntt_mul_(c, y, m, log_n, batch, p, g)
+    assert np.array_equal(host(y), oracle.vec_mul(p, X, host(m)))
+    del y, m
+    ops.ntt_(c, x, log_n, batch, True, p, g)
+    assert np.array_equal(host(x), a)
+
+
+def _context_with(env):
+    import os
+    import torch
+    from ronkathon_b200 import Context
+    old = {k: os.environ.get(k) for k in env}
+    os.environ.update(env)
+    try:
+        return Context(0, torch.cuda.current_stream().cuda_stream)
+    finally:
+        for k, v in old.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def test_montgomery_opt_in_variants_agree_with_the_default():
+    """The n-word inter-pass twiddle table (RONK_TW_TABLE=1: interpass_table<MontField>, twiddles in Montgomery form)
+    and launches without programmatic dependent launch (RONK_PDL=0) reproduce the default context's Montgomery
+    transforms bit for bit, with a prime above 2^63: forward, fused multiply and inverse at 2^20 and 2^24."""
+    import torch
+    from ronkathon_b200 import ops
+    c0 = ctx()
+    p, g = PBIG, 3
+    ref = {}
+    for lg in (20, 24):
+        a = ops.splitmix_fill(c0, 1 << lg, 31 + lg, p)
+        m = ops.splitmix_fill(c0, 1 << lg, 41 + lg, p)
+        x = a.clone()
+        ops.ntt_(c0, x, lg, 1, False, p, g)
+        y = a.clone()
+        ops.ntt_mul_(c0, y, m, lg, 1, p, g)
+        z = x.clone()
+        ops.ntt_(c0, z, lg, 1, True, p, g)
+        c0.sync()
+        assert torch.equal(z, a)
+        ref[lg] = (a, m, x, y)
+    for env in ({"RONK_TW_TABLE": "1"}, {"RONK_PDL": "0"}):
+        c1 = _context_with(env)
+        for lg, (a, m, x0, y0) in ref.items():
+            x = a.clone()
+            ops.ntt_(c1, x, lg, 1, False, p, g)
+            y = a.clone()
+            ops.ntt_mul_(c1, y, m, lg, 1, p, g)
+            z = x.clone()
+            ops.ntt_(c1, z, lg, 1, True, p, g)
+            c1.sync()
+            assert torch.equal(x, x0) and torch.equal(y, y0) and torch.equal(z, a), (env, lg)
+        c1.close()
+
+
+def _edge_cases():
+    gl = [("gl", lg, 1) for lg in range(1, 16)]                         # single tile 2^1 … 2^13; two-pass 2^14, 2^15
+    gl += [("gl", 16, 1), ("gl", 16, 2), ("gl", 16, 3)]                 # cluster kernel (batch ≤ 2), 256-point tiles
+    gl += [("gl", lg, 1) for lg in range(17, 27)]                       # split, 2^20, mid, 2^24, split over 2^24
+    return gl + [("pbig", lg, 1) for lg in (1, 4, 9, 13, 14, 16, 19, 22, 24, 26)]
+
+
+@pytest.mark.parametrize("name,log_n,batch", _edge_cases())
+def test_exact_edge_inputs_through_every_dispatch_branch(name, log_n, batch):
+    """Inputs at the edge of the range whose transforms are known exactly, at full length, through every branch of
+    run_ntt for Goldilocks (g = 7) and through the Montgomery kernels with a prime above 2^63:
+    all p - 1 → X[0] = -n, the rest 0; the inverse of all c → [c, 0, …, 0]; p - 1 at odd j → X[0] = -n/2, X[n/2] = n/2,
+    the rest 0; an impulse at j = 1 / j = n - 1 → X[k] = ω^(±k) (the powers kernel, itself spot-checked against the
+    oracle); a fused multiply by all p - 1 → -X."""
+    import torch
+    from ronkathon_b200 import _lib, ops
+    c = ctx()
+    p, g = (GL, 7) if name == "gl" else (PBIG, 3)
+    n, total = 1 << log_n, batch << log_n
+
+    def ntt(t, inverse=False, mul=None):
+        if mul is None:
+            ops.ntt_(c, t, log_n, batch, inverse, p, g)
+        else:
+            ops.ntt_mul_(c, t, mul, log_n, batch, p, g)
+        return t.view(batch, n)
+
+    def full(v):
+        return torch.full((total,), s64(v), dtype=torch.int64, device="cuda")
+
+    def want(*pairs):
+        e = torch.zeros((batch, n), dtype=torch.int64, device="cuda")
+        for k, v in pairs:
+            e[:, k] = s64(v % p)
+        return e
+
+    assert torch.equal(ntt(full(p - 1)), want((0, -n)))
+    assert torch.equal(ntt(full(p - 2), inverse=True), want((0, p - 2)))
+    alt = torch.zeros(total, dtype=torch.int64, device="cuda")
+    alt[1::2] = s64(p - 1)
+    assert torch.equal(ntt(alt), want((0, -(n // 2)), (n // 2, n // 2)))
+    w = oracle.root_of_unity(p, n, g)
+    for j, root in ((1, w), (n - 1, oracle.inverse(p, w))):
+        imp = torch.zeros((batch, n), dtype=torch.int64, device="cuda")
+        imp[:, j] = 1
+        pw = torch.empty(n, dtype=torch.int64, device="cuda")
+        c.call("ronk_field_powers_u64", p, root, 1, _lib._ptr(pw), n)
+        pwh = host(pw)
+        for k in sorted({0, 1, n // 2, n // 3, n - 1}):
+            assert int(pwh[k]) == oracle.pow_(p, root, k), (j, k)
+        assert torch.equal(ntt(imp.view(-1)), pw.expand(batch, n)), j
+    a = ops.splitmix_fill(c, total, 60 + log_n, p)
+    X = host(ntt(a.clone()))
+    negX = np.where(X == 0, np.uint64(0), np.uint64(p) - X)
+    assert np.array_equal(host(ntt(a, mul=full(p - 1))), negX)
+
+
+@pytest.mark.parametrize("name,log_l", [("gl", 21), ("gl", 22), ("gl", 23), ("gl", 24), ("pbig", 21), ("pbig", 24)])
+def test_poly_mul_of_all_minus_one_operands_is_the_trapezoid(name, log_l):
+    """poly_mul with 2^21 … 2^24-point transforms (Goldilocks: the bounded 256-point-tile route; the prime above 2^63: the
+    bounded Montgomery two-pass route).  Two all-(p - 1) operands multiply like two all-ones operands, so coefficient i
+    of the product is min(i + 1, da, db, da + db - 1 - i), exactly."""
+    from ronkathon_b200 import ops
+    c = ctx()
+    p, g = (GL, 7) if name == "gl" else (PBIG, 3)
+    L = (1 << log_l) - 5 if log_l < 24 else (1 << 24) - 1
+    da = L // 3 + 7
+    db = L + 1 - da
+    a = dev(np.full(da, p - 1, dtype=np.uint64))
+    b = dev(np.full(db, p - 1, dtype=np.uint64))
+    got = host(ops.poly_mul(c, a, b, p, g))
+    i = np.arange(L, dtype=np.uint64)
+    exp = np.minimum(np.minimum(i + np.uint64(1), np.uint64(min(da, db))), np.uint64(L) - i)
+    assert len(got) == L and np.array_equal(got, exp)
 
 
 def test_golden_vectors(gold64):
@@ -424,7 +599,8 @@ def test_virtual_rank_distributed_transform(log_g):
     c = ctx()
     G = 1 << log_g
     cases = [(GL, 7, max(2 * log_g, 4), 1), (GL, 7, 12, 3), (GL, 7, 16 + log_g, 2), (GL, 7, 20, 1), (GL, 7, 21 + log_g, 1),
-             (2013265921, 31, 10, 2), (GL, pow(7, 5, GL), 12, 2)]
+             (2013265921, 31, 10, 2), (GL, pow(7, 5, GL), 12, 2),
+             (PBIG, 3, 20 + log_g, 1), (BABYBEAR, 31, 16 + log_g, 2)]   # shared multiplier through the Montgomery two-pass kernel
     for p, g, log_n, batch in cases:
         n, m = 1 << log_n, (1 << log_n) // G
         blk = m // G

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import oracle
-from gpu_util import GL, ctx, dev, host
+from gpu_util import BABYBEAR, GL, MONT_PRIMES, PBIG, ctx, dev, host
 
 pytestmark = pytest.mark.gpu
 
@@ -50,7 +50,7 @@ def test_lagrange_evaluate_matches_oracle_including_node_quirk():
 
 
 def test_divrem_random_and_panics():
-    from ronkathon_b200 import PlutoBaseField, PlutoScalarField, Polynomial, RonkPanic
+    from ronkathon_b200 import PlutoBaseField, PlutoScalarField, Polynomial, PrimeField, RonkPanic
     ctx()
     rng = np.random.default_rng(4)
     for F, p in ((PlutoBaseField, 101), (PlutoScalarField, 17)):
@@ -61,6 +61,15 @@ def test_divrem_random_and_panics():
             q, r = Polynomial(a, F).quotient_and_remainder(Polynomial(b, F))
             eq, er = oracle.poly_divrem(p, a, b)
             assert list(q.coefficients) == list(eq) and list(r.coefficients) == list(er)
+    for p in (PBIG, BABYBEAR):                                  # Montgomery moduli above 2^63 and below 2^31
+        F = PrimeField(p)
+        for da, db in ((9, 3), (6, 6), (12, 2), (4, 7), (40, 5)):
+            a, b = oracle.splitmix(p, 30 + da, da), oracle.splitmix(p, 40 + db, db)
+            b[-1] = b[-1] or 1
+            a[0], b[0] = p - 1, p - 2
+            q, r = Polynomial(a, F).quotient_and_remainder(Polynomial(b, F))
+            eq, er = oracle.poly_divrem(p, a, b)
+            assert np.array_equal(q.coefficients, eq) and np.array_equal(r.coefficients, er), (p, da, db)
     with pytest.raises(RonkPanic):
         Polynomial([1, 2, 3], PlutoBaseField) / Polynomial([0, 0], PlutoBaseField)
     with pytest.raises(oracle.OraclePanic):
@@ -77,10 +86,11 @@ def test_div_by_linear_factor_scan_vs_oracle_and_identity():
     """§8f row 1: Polynomial::div/rem by the divisor kzg::open builds (kzg/setup.rs:72-75) runs as a
     device-wide scan.  Bit-exact vs the literal long division of the oracle (mod.rs:170-225) at sizes
     it finishes, and a = q·(b0 + b1·x) + r coefficient by coefficient at 2^22."""
-    from ronkathon_b200 import GoldilocksField, PlutoBaseField, PlutoScalarField, Polynomial
+    from ronkathon_b200 import GoldilocksField, PlutoBaseField, PlutoScalarField, Polynomial, PrimeField
     c = ctx()
     rng = np.random.default_rng(11)
-    for F, p in ((PlutoBaseField, 101), (PlutoScalarField, 17), (GoldilocksField, GL)):
+    for F, p in ((PlutoBaseField, 101), (PlutoScalarField, 17), (GoldilocksField, GL), (PrimeField(PBIG), PBIG),
+                 (PrimeField(BABYBEAR), BABYBEAR)):
         for d in (1, 2, 3, 15, 16, 17, 255, 4095, 4096, 4097, 8193, 9001):
             a = oracle.splitmix(p, 100 + d, d)
             for b in ([int(rng.integers(0, p, dtype=np.uint64)), 1],
@@ -97,18 +107,19 @@ def test_div_by_linear_factor_scan_vs_oracle_and_identity():
     assert np.array_equal(q.coefficients[:-1], base) and q.coefficients[-1] == 0 and not r.coefficients.any()
     # device-pointer entry at 2^22 (1024 chunks): identity check, remainder = a(z) by the evaluate kernel
     d = 1 << 22
-    a = oracle.splitmix(GL, 77, d)
-    b0, b1 = 1234567890123456789 % GL, 987654321987654321 % GL
-    A, Q, R = dev(a), dev(np.zeros(d, np.uint64)), dev(np.zeros(1, np.uint64))
-    c.call("ronk_poly_div_linear_u64", GL, A.data_ptr(), d, b0, b1, Q.data_ptr(), R.data_ptr())
-    q, r = host(Q), host(R)
-    assert q[-1] == 0
-    recomposed = oracle.poly_add(GL, oracle.vec_mul(GL, q, np.full(d, b0, np.uint64)),
-                                 np.concatenate([np.zeros(1, np.uint64), oracle.vec_mul(GL, q, np.full(d, b1, np.uint64))[:-1]]))
-    recomposed[0] = oracle.add(GL, int(recomposed[0]), int(r[0]))
-    assert np.array_equal(recomposed, a)
-    zpt = oracle.mul(GL, GL - b0, oracle.inverse(GL, b1))
-    assert int(r[0]) == oracle.poly_eval_horner(GL, a, zpt)
+    for p in (GL, PBIG, BABYBEAR):
+        a = oracle.splitmix(p, 77, d)
+        b0, b1 = 1234567890123456789 % p, 987654321987654321 % p
+        A, Q, R = dev(a), dev(np.zeros(d, np.uint64)), dev(np.zeros(1, np.uint64))
+        c.call("ronk_poly_div_linear_u64", p, A.data_ptr(), d, b0, b1, Q.data_ptr(), R.data_ptr())
+        q, r = host(Q), host(R)
+        assert q[-1] == 0
+        recomposed = oracle.poly_add(p, oracle.vec_mul(p, q, np.full(d, b0, np.uint64)),
+                                     np.concatenate([np.zeros(1, np.uint64), oracle.vec_mul(p, q, np.full(d, b1, np.uint64))[:-1]]))
+        recomposed[0] = oracle.add(p, int(recomposed[0]), int(r[0]))
+        assert np.array_equal(recomposed, a), p
+        zpt = oracle.mul(p, p - b0, oracle.inverse(p, b1))
+        assert int(r[0]) == oracle.poly_eval_horner(p, a, zpt), p
     with pytest.raises(Exception):
         c.call("ronk_poly_div_linear_u64", GL, A.data_ptr(), d, b0, 0, Q.data_ptr(), R.data_ptr())
     with pytest.raises(Exception):
@@ -133,7 +144,15 @@ def test_reed_solomon_decode_interpolation(kats):
             ys = [int(v) for v in oracle.splitmix(p, 60 + k, k)]
             got = codes.rs_decode(list(zip(xs, ys)), k, F)
             assert [v.value for v in got] == [int(v) for v in oracle.rs_decode(p, xs, ys, k)], (p, k)
-    for n in (256, 2048):                                                # full root-of-unity set: ifft
+    from ronkathon_b200 import _lib
+    for p in (PBIG, BABYBEAR):                                           # Montgomery moduli, the C entry point directly
+        for k in (1, 2, 3, 6, 10):
+            xs, ys = oracle.splitmix(p, 50 + k, k), oracle.splitmix(p, 60 + k, k)
+            ys[0] = p - 1
+            out = np.empty(k, dtype=np.uint64)
+            ctx().call("ronk_poly_interpolate_u64_host", p, _lib._ptr(xs), _lib._ptr(ys), k, _lib._ptr(out))
+            assert np.array_equal(out, oracle.rs_decode(p, xs, ys, k)), (p, k)
+    for n in (256, 2048):                                              # full root-of-unity set: ifft
         msg = oracle.splitmix(GL, n, n)
         w = oracle.root_of_unity(GL, n)
         xs = np.array([pow(w, i, GL) for i in range(n)], dtype=np.uint64)
@@ -258,14 +277,17 @@ def test_evaluate_vs_oracle(gold64):
     a3 = oracle.splitmix(GL, 42, 300)
     e = gold64["eval_300_seed42_at_seed43_0"]
     assert Polynomial(a3, GoldilocksField).evaluate(e["x"]).value == e["y"]
-    for d in (0, 1, 2, 255, 256, 257, 1000, 70000):
-        co = oracle.splitmix(GL, d + 5, d)
-        xs = np.concatenate([oracle.splitmix(GL, 8, 5), np.array([0, 1, GL - 1], dtype=np.uint64)])
-        got = host(ops.poly_eval(c, dev(co) if d else dev(np.zeros(1, np.uint64))[:0], dev(xs)))
-        exp = [oracle.poly_eval_horner(GL, co, int(x)) if d else 0 for x in xs]
-        assert list(got) == exp, d
-        if 0 < d <= 300:  # the reference's literal O(D²) form gives the same values
-            assert exp == [oracle.poly_eval(GL, co, int(x)) for x in xs]
+    for p in (GL, PBIG, BABYBEAR):
+        for d in (0, 1, 2, 255, 256, 257, 1000, 70000):
+            co = oracle.splitmix(p, d + 5, d)
+            if d:
+                co[-1] = p - 1
+            xs = np.concatenate([oracle.splitmix(p, 8, 5), np.array([0, 1, p - 1], dtype=np.uint64)])
+            got = host(ops.poly_eval(c, dev(co) if d else dev(np.zeros(1, np.uint64))[:0], dev(xs), p))
+            exp = [oracle.poly_eval_horner(p, co, int(x)) if d else 0 for x in xs]
+            assert list(got) == exp, (p, d)
+            if 0 < d <= 300:  # the reference's literal O(D²) form gives the same values
+                assert exp == [oracle.poly_eval(p, co, int(x)) for x in xs]
 
 
 def test_reed_solomon_encode_and_shamir_next_rows(kats):
@@ -286,3 +308,54 @@ def test_reed_solomon_encode_and_shamir_next_rows(kats):
     assert [x.value for x, _ in cw] == list(xs) and [y.value for _, y in cw] == list(ys)
     shares = codes.shamir_shares([11, 5, 7, 3], 9, PrimeField(101))
     assert [(x, y.value) for x, y in shares] == [(x, oracle.poly_eval(101, [11, 5, 7, 3], x)) for x in range(1, 10)]
+
+
+def _conv_oracle(p, g, a, b):
+    """The product by the convolution theorem with the oracle's transforms."""
+    L = len(a) + len(b) - 1
+    n = 1 << (L - 1).bit_length()
+    pa, pb = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+    pa[:len(a)], pb[:len(b)] = a, b
+    return oracle.ntt_fast(p, oracle.vec_mul(p, oracle.ntt_fast(p, pa, g=g), oracle.ntt_fast(p, pb, g=g)), inverse=True, g=g)[:L]
+
+
+def _poly_mul_generic_cases():
+    cases = [(name, 64, 64) for name in MONT_PRIMES] + [(name, 200, 200) for name in MONT_PRIMES]   # schoolbook | NTT
+    for name in ("babybear", "pbig"):                       # transforms of 2^13 … 2^20 points: single tile, two-pass
+        cases += [(name, (1 << (k - 2)) + 5, (1 << (k - 1)) - 17) for k in range(13, 21)]
+    cases += [("koalabear", 5000, 9000), ("p32", 40000, 25000), ("p57", 30001, 2), ("gl_g5", 70000, 60000)]
+    return cases
+
+
+@pytest.mark.parametrize("name,da,db", _poly_mul_generic_cases())
+def test_poly_mul_generic_primes_vs_oracle(name, da, db):
+    """poly_mul with every (p, g) of the Montgomery table: both sides of the schoolbook / NTT crossover against the
+    oracle's schoolbook product, and products whose transforms have 2^13 … 2^20 points (the bounded single-tile and
+    bounded two-pass Montgomery kernels, fused multiply included) against the oracle's convolution-theorem route."""
+    from ronkathon_b200 import ops
+    c = ctx()
+    p, g, _ = MONT_PRIMES[name]
+    a, b = oracle.splitmix(p, 300 + da, da), oracle.splitmix(p, 400 + db, db)
+    a[0], b[-1] = p - 1, p - 2
+    got = host(ops.poly_mul(c, dev(a), dev(b), p, g))
+    exp = oracle.poly_mul(p, a, b) if da * db <= 100_000 else _conv_oracle(p, g, a, b)
+    assert np.array_equal(got, exp), (name, da, db)
+
+
+@pytest.mark.parametrize("name,da,db", [("babybear", (1 << 22) + 3, (1 << 22) - 9), ("pbig", 1 << 23, 1 << 23),
+                                        ("p32", (1 << 15) + 1, (1 << 15) + 1)])
+def test_poly_mul_generic_primes_large_and_beyond_the_two_adicity(name, da, db):
+    """Products of 2^23 and 2^24 points on the Montgomery two-pass kernels, and one too long for the prime's 2-adicity
+    (2^15 + 1 squared needs 2^17 points, 4295294977 has 2^16), which falls back to schoolbook: the length, the end
+    coefficients and c(x) = a(x)·b(x) at random points by the oracle's Horner evaluation."""
+    from ronkathon_b200 import ops
+    c = ctx()
+    p, g, _ = MONT_PRIMES[name]
+    A, B = ops.splitmix_fill(c, da, 500, p), ops.splitmix_fill(c, db, 501, p)
+    got, a, b = host(ops.poly_mul(c, A, B, p, g)), host(A), host(B)
+    assert len(got) == da + db - 1
+    assert int(got[0]) == oracle.mul(p, int(a[0]), int(b[0])) and int(got[-1]) == oracle.mul(p, int(a[-1]), int(b[-1]))
+    for x in oracle.splitmix(p, 502, 4):
+        x = int(x)
+        assert oracle.poly_eval_horner(p, got, x) == oracle.mul(p, oracle.poly_eval_horner(p, a, x),
+                                                                oracle.poly_eval_horner(p, b, x)), (name, x)

@@ -10,8 +10,9 @@ import numpy as np
 import pytest
 
 import oracle
+from gpu_util import BABYBEAR, PBIG
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+HERE =os.path.dirname(os.path.abspath(__file__))
 GL = oracle.GOLDILOCKS
 P64 = C.POINTER(C.c_uint64)
 
@@ -178,6 +179,13 @@ def test_emulated_two_pass_generic_and_fused_mul(emu, gold64):
     A10 = emu_ntt(emu, GL, 7, a10, 10)
     exp = np.array([oracle.mul(GL, int(x), int(y)) for x, y in zip(oracle.ntt_fast(GL, b10), A10)], dtype=np.uint64)
     assert np.array_equal(emu_ntt(emu, GL, 7, b10, 10, mul=A10), exp)
+    # Montgomery fused multiply in the pass-2 store, with the preferred and the adapted tile shapes
+    for p, g, lg in ((PBIG, 3, 16), (BABYBEAR, 31, 18)):
+        x, m = oracle.splitmix(p, 44, 1 << lg), oracle.splitmix(p, 45, 1 << lg)
+        x[0], m[1] = p - 1, p - 1
+        exp = oracle.vec_mul(p, oracle.ntt_fast(p, x, g=g), m)
+        for tiles in ((14, 13), (12, 11)):
+            assert np.array_equal(emu_ntt(emu, p, g, x, lg, mul=m, tiles=tiles), exp), (p, lg, tiles)
 
 
 def emu_ntt_bounded(emu, p, g, src, dst_len, log_n, inverse=False, mul=None, tile_cap=12, tiles=(13, 13)):
@@ -194,6 +202,9 @@ def emu_ntt_bounded(emu, p, g, src, dst_len, log_n, inverse=False, mul=None, til
     (GL, 7, 3, 5, 8), (GL, 7, 10, 1, 1024), (GL, 7, 12, 3000, 4000), (GL, 7, 13, 4097, 8191),
     (GL, 7, 14, 8192, 16383), (GL, 7, 15, 20001, 32768), (GL, 7, 16, 32768, 65535), (GL, 7, 16, 65536, 17),
     (17, 14, 4, 7, 13), (GL, 49, 14, 5000, 9000),
+    (BABYBEAR, 31, 15, 20001, 32768), (BABYBEAR, 31, 16, 65536, 40001), (BABYBEAR, 31, 17, 70000, 131071),
+    (BABYBEAR, 31, 18, 131073, 262144), (PBIG, 3, 15, 32768, 20000), (PBIG, 3, 16, 30001, 65536),
+    (PBIG, 3, 17, 131072, 99999), (PBIG, 3, 18, 200001, 262143),
 ])
 @pytest.mark.parametrize("variant", [0, 1, 2])
 def test_emulated_bounded_out_of_place_transform(emu, p, g, log_n, src_len, dst_len, variant):
@@ -217,10 +228,10 @@ def _bounded_checks(emu, p, g, log_n, src, padded, dst_len):
         keep = src.copy()
         got = emu_ntt_bounded(emu, p, g, src, dst_len, log_n, inverse=inverse)
         assert np.array_equal(got, ref[:dst_len]) and np.array_equal(src, keep), (log_n, inverse)
-    if p == GL and g == 7:  # with the fused point-wise multiply (the second transform of poly_mul)
-        mul = oracle.splitmix(p, 77, n)
-        got = emu_ntt_bounded(emu, p, g, src, n, log_n, mul=mul)
-        assert np.array_equal(got, oracle.vec_mul(p, oracle.ntt_fast(p, padded), mul))
+    # with the fused point-wise multiply (the second transform of poly_mul)
+    mul = oracle.splitmix(p, 77, n)
+    got = emu_ntt_bounded(emu, p, g, src, n, log_n, mul=mul)
+    assert np.array_equal(got, oracle.vec_mul(p, oracle.ntt_fast(p, padded, g=g), mul))
 
 
 # ---- the specialised 4096-point-per-tile kernel (ntt12_kernel.cuh) ------------------------------------------
