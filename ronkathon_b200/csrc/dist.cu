@@ -279,35 +279,15 @@ static int dist_twcol(ronk_ctx* ctx, DistState* d, u64 p, u64 g, u32 log_n, cons
   return RONK_OK;
 }
 
-template <class F>
-static int launch_cross(ronk_ctx* ctx, const F& f, u32 log_g, const PeerPtrs& src, u64* out, size_t blk, u32 batch,
-                        size_t bstride, size_t off, size_t ostride) {
-  const size_t total = (size_t)batch * blk;
-  size_t blocks = (total + 255) / 256;
-  const size_t cap = (size_t)ctx->sm_count * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  LaunchScope ls(ctx, "ntt_cross_rank");
-  switch (log_g) {
-    case 1: cross_rank_kernel<F, 1><<<(unsigned)blocks, 256, 0, ctx->stream>>>(f, src, out, blk, batch, bstride, off, ostride); break;
-    case 2: cross_rank_kernel<F, 2><<<(unsigned)blocks, 256, 0, ctx->stream>>>(f, src, out, blk, batch, bstride, off, ostride); break;
-    case 3: cross_rank_kernel<F, 3><<<(unsigned)blocks, 256, 0, ctx->stream>>>(f, src, out, blk, batch, bstride, off, ostride); break;
-    default: cross_rank_kernel<F, 4><<<(unsigned)blocks, 256, 0, ctx->stream>>>(f, src, out, blk, batch, bstride, off, ostride); break;
-  }
-  return RONK_OK;
-}
-
 static int cross_rank(ronk_ctx* ctx, u64 p, u64 g, u32 log_g, const PeerPtrs& src, u64* out, size_t blk, u32 batch,
                       size_t bstride, size_t off, size_t ostride) {
-  if (is_goldilocks_fast(p, g)) {
-    GoldilocksField f;
-    RONK_TRY(launch_cross(ctx, f, log_g, src, out, blk, batch, bstride, off, ostride));
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, g, false, &f));
-    RONK_TRY(launch_cross(ctx, f, log_g, src, out, blk, batch, bstride, off, ostride));
-  }
-  return check_launch(ctx, "cross_rank_kernel");
+  const int blocks = grid_for(ctx, (size_t)batch * blk, 256);
+  return with_field(ctx, p, g, false, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    auto kernel = log_g == 1 ? cross_rank_kernel<F, 1> : log_g == 2 ? cross_rank_kernel<F, 2>
+                : log_g == 3 ? cross_rank_kernel<F, 3> : cross_rank_kernel<F, 4>;
+    return launch(ctx, "ntt_cross_rank", kernel, blocks, 256, 0, false, f, src, out, blk, batch, bstride, off, ostride);
+  });
 }
 
 }  // namespace ronk
@@ -460,14 +440,8 @@ int ronk_ntt_u64_dist(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* local, ui
   RONK_TRY(ntt_device_shared_mul(ctx, p, g, (const u64*)local, (u64*)local, twcol, log_m, batch));
   const u64* sendbase = (const u64*)local;
   if (batch > 1) {  // the block for destination s is strided over the batch: make it contiguous first
-    size_t blocks = (words + 255) / 256;
-    const size_t cap = (size_t)ctx->sm_count * 16;
-    if (blocks > cap) blocks = cap;
-    {
-      LaunchScope ls(ctx, "dist_pack");
-      pack_blocks_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>((const u64*)local, d->pack, blk, lg, batch);
-    }
-    RONK_TRY(check_launch(ctx, "pack_blocks_kernel"));
+    RONK_TRY(launch(ctx, "dist_pack", pack_blocks_kernel, grid_for(ctx, words, 256, 16), 256, 0, false, (const u64*)local, d->pack,
+                    blk, lg, batch));
     sendbase = d->pack;
   }
   const size_t chunk = (size_t)batch * blk;  // words per (source, destination) pair
@@ -525,14 +499,8 @@ int ronk_ntt_u64_dist_virtual(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* d
       RONK_TRY(ntt_device_shared_mul(ctx, p, g, local, local, twcol, log_m, batch));
       const u64* sendbase = local;
       if (batch > 1) {
-        size_t blocks = (words + 255) / 256;
-        const size_t cap = (size_t)ctx->sm_count * 16;
-        if (blocks > cap) blocks = cap;
-        {
-          LaunchScope ls(ctx, "dist_pack");
-          pack_blocks_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(local, sc.pack, blk, log_g, batch);
-        }
-        RONK_TRY(check_launch(ctx, "pack_blocks_kernel"));
+        RONK_TRY(launch(ctx, "dist_pack", pack_blocks_kernel, grid_for(ctx, words, 256, 16), 256, 0, false, local, sc.pack, blk,
+                        log_g, batch));
         sendbase = sc.pack;
       }
       // the all-to-all: source r's chunk for destination s lands in s's receive buffer at slot r
@@ -580,11 +548,7 @@ int ronk_msm_pluto_ext_dist(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   u32* host_dev = nullptr;
   RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&host_dev, (void*)ctx->h_flag, 0));
   host[1] = PT_INF;
-  {
-    LaunchScope ls(ctx, "point_sum");
-    point_sum_kernel<<<1, 32, 0, ctx->stream>>>(d->gather, (u32)d->world, (volatile u32*)(host_dev + 1));
-  }
-  RONK_TRY(check_launch(ctx, "point_sum_kernel"));
+  RONK_TRY(launch(ctx, "point_sum", point_sum_kernel, 1, 32, 0, false, d->gather, (u32)d->world, host_dev + 1));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   const u32 res = host[1];
   out[0] = (uint8_t)(res & 0xFF);

@@ -141,14 +141,6 @@ int validate_modulus(ronk_ctx* ctx, u64 p) {
   return RONK_OK;
 }
 
-static int grid_for(ronk_ctx* ctx, size_t n, int threads) {
-  size_t blocks = (n + threads - 1) / threads;
-  size_t cap = (size_t)ctx->sm_count * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks == 0) blocks = 1;
-  return (int)blocks;
-}
-
 static int reset_flag(ronk_ctx* ctx) {
   RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
   return RONK_OK;
@@ -166,18 +158,10 @@ static int binop(ronk_ctx* ctx, u64 p, const u64* a, const u64* b, u64* out, siz
   RONK_TRY(validate_modulus(ctx, p));
   if (n == 0) return RONK_OK;
   if (OP == OP_DIV) RONK_TRY(reset_flag(ctx));
-  const int threads = 256, blocks = grid_for(ctx, n, threads);
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, name);
-    binop_kernel<GoldilocksField, OP><<<blocks, threads, 0, ctx->stream>>>(f, a, b, out, n, ctx->d_flag);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, name);
-    binop_kernel<MontField, OP><<<blocks, threads, 0, ctx->stream>>>(f, a, b, out, n, ctx->d_flag);
-  }
-  RONK_TRY(check_launch(ctx, name));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, name, binop_kernel<std::decay_t<decltype(f)>, OP>, grid_for(ctx, n, 256), 256, 0, false, f, a, b,
+                  out, n, ctx->d_flag);
+  }));
   if (OP == OP_DIV) {
     int v = 0;
     RONK_TRY(read_flag(ctx, &v));
@@ -192,18 +176,10 @@ static int unop(ronk_ctx* ctx, u64 p, const u64* a, u64* out, size_t n, u64 e, c
   RONK_TRY(validate_modulus(ctx, p));
   if (n == 0) return RONK_OK;
   if (OP == UOP_INV) RONK_TRY(reset_flag(ctx));
-  const int threads = 256, blocks = grid_for(ctx, n, threads);
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, name);
-    unop_kernel<GoldilocksField, OP><<<blocks, threads, 0, ctx->stream>>>(f, a, out, n, e, ctx->d_flag);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, name);
-    unop_kernel<MontField, OP><<<blocks, threads, 0, ctx->stream>>>(f, a, out, n, e, ctx->d_flag);
-  }
-  RONK_TRY(check_launch(ctx, name));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, name, unop_kernel<std::decay_t<decltype(f)>, OP>, grid_for(ctx, n, 256), 256, 0, false, f, a, out,
+                  n, e, ctx->d_flag);
+  }));
   if (OP == UOP_INV) {
     int v = 0;
     RONK_TRY(read_flag(ctx, &v));
@@ -282,18 +258,10 @@ int ronk_field_powers_u64(ronk_ctx* ctx, uint64_t p, uint64_t base, uint64_t sca
   RONK_TRY(validate_modulus(ctx, p));
   if (base >= p || scale >= p) return set_err(ctx, RONK_EINVAL, "non-canonical argument");
   if (n == 0) return RONK_OK;
-  const int threads = 256, blocks = grid_for(ctx, (n + 7) / 8, threads);
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "field_powers");
-    powers_kernel<GoldilocksField><<<blocks, threads, 0, ctx->stream>>>(f, base, scale, (u64*)out, n);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, "field_powers");
-    powers_kernel<MontField><<<blocks, threads, 0, ctx->stream>>>(f, base, scale, (u64*)out, n);
-  }
-  return check_launch(ctx, "powers_kernel");
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "field_powers", powers_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, (n + 7) / 8, 256), 256, 0,
+                  false, f, base, scale, (u64*)out, n);
+  });
 }
 
 int ronk_ntt_strided_small_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* data, uint32_t log_g, size_t stride,
@@ -314,20 +282,10 @@ int ronk_ntt_strided_small_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* 
   RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 16 * sizeof(u64)));
   RONK_CUDA(ctx, cudaMemcpyAsync(ctx->ws2, h_wt, G * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_wt is a stack buffer
-  const int threads = 128, blocks = grid_for(ctx, count, threads);
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "ntt_cross_rank");
-    strided_dft_kernel<GoldilocksField><<<blocks, threads, 0, ctx->stream>>>(f, (u64*)data, (u32)G, stride, count,
-                                                                             (const u64*)ctx->ws2, sc);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, "ntt_cross_rank");
-    strided_dft_kernel<MontField><<<blocks, threads, 0, ctx->stream>>>(f, (u64*)data, (u32)G, stride, count,
-                                                                       (const u64*)ctx->ws2, sc);
-  }
-  return check_launch(ctx, "strided_dft_kernel");
+  return with_field(ctx, p, 0, false, [&](const auto& f) {  // the transform's roots come from the wt table, not the policy
+    return launch(ctx, "ntt_cross_rank", strided_dft_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, count, 128), 128, 0,
+                  false, f, (u64*)data, (u32)G, stride, count, (const u64*)ctx->ws2, sc);
+  });
 }
 
 int ronk_ntt_cross_rank_fused_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* const* peer_bufs,
@@ -359,31 +317,17 @@ int ronk_ntt_cross_rank_fused_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const u
   for (u32 r = 0; r < 16; r++) pp.p[r] = r < G ? (const u64*)peer_bufs[r] : nullptr;
   for (u32 r = 0; r < G; r++)
     if (!pp.p[r]) return set_err(ctx, RONK_EINVAL, "null peer buffer");
-  const int threads = 128;
-  size_t blocks = (blk + threads - 1) / threads;
-  if (blocks > (size_t)ctx->sm_count * 16) blocks = (size_t)ctx->sm_count * 16;
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "ntt_cross_rank_fused");
-    cross_rank_fused_kernel<GoldilocksField><<<(int)blocks, threads, 0, ctx->stream>>>(f, pp, d_tw, d_wt, (u64*)out, G, blk, rank);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, "ntt_cross_rank_fused");
-    cross_rank_fused_kernel<MontField><<<(int)blocks, threads, 0, ctx->stream>>>(f, pp, d_tw, d_wt, (u64*)out, G, blk, rank);
-  }
-  return check_launch(ctx, "cross_rank_fused_kernel");
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "ntt_cross_rank_fused", cross_rank_fused_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, blk, 128, 16),
+                  128, 0, false, f, pp, d_tw, d_wt, (u64*)out, G, blk, rank);
+  });
 }
 
 int ronk_splitmix_fill_u64(ronk_ctx* ctx, uint64_t p, uint64_t seed, uint64_t* out, size_t n) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || (n && !out) || p == 0) return set_err(ctx, RONK_EINVAL, "bad argument");
   if (n == 0) return RONK_OK;
-  {
-    LaunchScope ls(ctx, "splitmix_fill");
-    splitmix_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->stream>>>(p, seed, (u64*)out, n);
-  }
-  return check_launch(ctx, "splitmix_kernel");
+  return launch(ctx, "splitmix_fill", splitmix_kernel, grid_for(ctx, n, 256), 256, 0, false, p, seed, (u64*)out, n);
 }
 
 // ---- host-pointer variants -------------------------------------------------------------------

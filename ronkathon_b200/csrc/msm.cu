@@ -435,21 +435,15 @@ static int msm_coord_device(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   static_assert((kTabWords + MSM_EXP * MSM_EXP) % 2 == 0, "the 64-bit accumulator must be 8-byte aligned");
   unsigned long long* gacc = (unsigned long long*)((u32*)ctx->msm_coord + kTabWords + MSM_EXP * MSM_EXP);
   // a CTA is worth its 82 KB table load once every thread sees ≥ 4 terms
-  size_t ctas = (n_scalars + (size_t)MSM_COORD_THREADS * 4 - 1) / ((size_t)MSM_COORD_THREADS * 4);
-  if (ctas > (size_t)ctx->sm_count) ctas = (size_t)ctx->sm_count;
-  if (ctas < 1) ctas = 1;
+  const int ctas = grid_for(ctx, n_scalars, MSM_COORD_THREADS * 4, 1);
   const int vec = (((uintptr_t)points & 15) == 0 && ((uintptr_t)scalars & 3) == 0) ? 1 : 0;
   volatile u32* host = (volatile u32*)ctx->h_flag;  // mapped pinned: [0] = flag, [1] = result
   host[0] = 0u;
   host[1] = PT_INF;
   u32* host_dev = nullptr;
   RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&host_dev, (void*)ctx->h_flag, 0));
-  {
-    LaunchScope ls(ctx, "msm_coord");
-    msm_coord_kernel<<<(unsigned)ctas, MSM_COORD_THREADS, kSmem, ctx->stream>>>((const u32*)points, scalars, n_scalars, vec, bintab,
-                                                                                pttab, gacc, (volatile u32*)host_dev);
-  }
-  RONK_TRY(check_launch(ctx, "msm_coord_kernel"));
+  RONK_TRY(launch(ctx, "msm_coord", msm_coord_kernel, ctas, MSM_COORD_THREADS, kSmem, false, (const u32*)points, scalars,
+                  n_scalars, vec, bintab, pttab, gacc, host_dev));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (host[0]) return set_err(ctx, RONK_EINVAL, "off-curve point, non-canonical coordinate or scalar >= 17");
   *h_result = host[1];
@@ -483,14 +477,6 @@ __global__ void point_op_kernel(int op, const u32* a, const u32* b, const uint8_
   }
 }
 
-static int msm_grid(ronk_ctx* ctx, size_t n) {
-  size_t ctas = (n + (size_t)MSM_THREADS * MSM_TERMS - 1) / ((size_t)MSM_THREADS * MSM_TERMS);
-  const size_t cap = (size_t)ctx->sm_count * 8;
-  if (ctas > cap) ctas = cap;
-  if (ctas < 1) ctas = 1;
-  return (int)ctas;
-}
-
 // Histogram path: result of the first n_scalars terms (kzg::commit).  Two launches, no memset, no memcpy:
 // the kernels write the error flag and the result into mapped pinned host memory.
 static int msm_hist_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars, size_t n_scalars,
@@ -519,9 +505,7 @@ static int msm_hist_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points
   RONK_TRY(ensure_smem_attr(ctx, msm_hist_kernel, (int)kSmem));
   // one CTA per SM at most; each thread should see ≥ 8 terms before another CTA (its table load and its 82 KB of
   // partial histogram) is worth it (≥ 32 terms per thread made 2^20 terms slower)
-  size_t ctas = (n_scalars + (size_t)MSM_HIST_THREADS * 8 - 1) / ((size_t)MSM_HIST_THREADS * 8);
-  if (ctas > (size_t)ctx->sm_count) ctas = (size_t)ctx->sm_count;
-  if (ctas < 1) ctas = 1;
+  const size_t ctas = grid_for(ctx, n_scalars, MSM_HIST_THREADS * 8, 1);
   constexpr u32 fin_ctas = (MSM_BINS + MSM_FIN_THREADS - 1) / MSM_FIN_THREADS;  // 80
   static_assert(fin_ctas <= MSM_FIN_THREADS, "final tree assumes one CTA sum per thread");
   const size_t need = (ctas * MSM_BINS + fin_ctas) * sizeof(u32);
@@ -535,33 +519,10 @@ static int msm_hist_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points
   host[1] = PT_INF;
   u32* host_dev = nullptr;
   RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&host_dev, (void*)ctx->h_flag, 0));
-  {
-    LaunchScope ls(ctx, "msm_hist");
-    msm_hist_kernel<<<(unsigned)ctas, MSM_HIST_THREADS, kSmem, ctx->stream>>>(
-        (const u32*)points, scalars, n_scalars, (const uint16_t*)ctx->msm_ytab, partial, ghist, (volatile int*)host_dev);
-  }
-  RONK_TRY(check_launch(ctx, "msm_hist_kernel"));
-  {
-    LaunchScope ls(ctx, "msm_hist_finish");
-    if (ctx->tune.pdl && !ctx->prof) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(fin_ctas);
-      cfg.blockDim = dim3(MSM_FIN_THREADS * MSM_FIN_GROUPS);
-      cfg.stream = ctx->stream;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      RONK_CUDA(ctx, cudaLaunchKernelEx(&cfg, msm_hist_finish_kernel, (const u32*)partial, (u32)ctas, ghist,
-                                        (const uint16_t*)ctx->msm_ytab, cta_sum, (u32*)ctx->msm_done,
-                                        (volatile u32*)(host_dev + 1)));
-    } else {
-      msm_hist_finish_kernel<<<fin_ctas, MSM_FIN_THREADS * MSM_FIN_GROUPS, 0, ctx->stream>>>(
-          partial, (u32)ctas, ghist, (const uint16_t*)ctx->msm_ytab, cta_sum, (u32*)ctx->msm_done, (volatile u32*)(host_dev + 1));
-    }
-  }
-  RONK_TRY(check_launch(ctx, "msm_hist_finish_kernel"));
+  RONK_TRY(launch(ctx, "msm_hist", msm_hist_kernel, (unsigned)ctas, MSM_HIST_THREADS, kSmem, false, (const u32*)points, scalars,
+                  n_scalars, (const uint16_t*)ctx->msm_ytab, partial, ghist, (volatile int*)host_dev));
+  RONK_TRY(launch(ctx, "msm_hist_finish", msm_hist_finish_kernel, fin_ctas, MSM_FIN_THREADS * MSM_FIN_GROUPS, 0, ctx->tune.pdl,
+                  partial, (u32)ctas, ghist, (const uint16_t*)ctx->msm_ytab, cta_sum, (u32*)ctx->msm_done, host_dev + 1));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (host[0]) return set_err(ctx, RONK_EINVAL, "off-curve point, non-canonical coordinate or scalar >= 17");
   *h_result = host[1];
@@ -575,7 +536,7 @@ static int msm_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, con
   if (!ctx || (n_scalars && (!points || !scalars))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n_points < n_scalars) return set_err(ctx, RONK_EINVAL, "srs shorter than coefficients (kzg/setup.rs:53)");
   if (((uintptr_t)points & 3) != 0) return set_err(ctx, RONK_EINVAL, "points must be 4-byte aligned");
-  const int ctas = msm_grid(ctx, n_scalars);
+  const int ctas = grid_for(ctx, n_scalars, MSM_THREADS * MSM_TERMS);
   // device block [flag | 17 buckets | result]: one memset, and one copy into pinned host memory at the end
   // (two copies into pageable memory cost a large share of a small call)
   const size_t need = ((size_t)ctas * 17 + 1 + 17 + 1) * sizeof(u32);
@@ -585,17 +546,10 @@ static int msm_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, con
   u32* d_buckets = d_mflag + 1;
   u32* d_result = d_buckets + 17;
   RONK_CUDA(ctx, cudaMemsetAsync(d_mflag, 0, sizeof(u32), ctx->stream));
-  {
-    LaunchScope ls(ctx, "msm_bucket");
-    msm_bucket_kernel<<<ctas, MSM_THREADS, 0, ctx->stream>>>((const u32*)points, scalars, n_scalars, partial,
-                                                            (int*)d_mflag);
-  }
-  RONK_TRY(check_launch(ctx, "msm_bucket_kernel"));
-  {
-    LaunchScope ls(ctx, "msm_finish");
-    msm_finish_kernel<<<1, 16 * MSM_FIN_LANES, 0, ctx->stream>>>(partial, (u32)ctas, d_buckets, d_result);
-  }
-  RONK_TRY(check_launch(ctx, "msm_finish_kernel"));
+  RONK_TRY(launch(ctx, "msm_bucket", msm_bucket_kernel, ctas, MSM_THREADS, 0, false, (const u32*)points, scalars, n_scalars,
+                  partial, (int*)d_mflag));
+  RONK_TRY(launch(ctx, "msm_finish", msm_finish_kernel, 1, 16 * MSM_FIN_LANES, 0, false, partial, (u32)ctas, d_buckets,
+                  d_result));
   u32* host = (u32*)ctx->h_flag;  // pinned, 32 words
   RONK_CUDA(ctx, cudaMemcpyAsync(host, d_mflag, 19 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -611,11 +565,6 @@ static void unpack_to_bytes(u32 w, uint8_t out[4]) {
   out[2] = (uint8_t)((w >> 16) & 0xFF);
   out[3] = (uint8_t)(w >> 24);
 }
-
-struct DevBytes {
-  void* p = nullptr;
-  ~DevBytes() { if (p) cudaFree(p); }
-};
 
 }  // namespace ronk
 
@@ -650,7 +599,7 @@ int ronk_msm_pluto_ext_host(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || !out || (n_scalars && (!points || !scalars))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n_points < n_scalars) return set_err(ctx, RONK_EINVAL, "srs shorter than coefficients (kzg/setup.rs:53)");
-  DevBytes P, S;
+  DevBuf P, S;
   RONK_CUDA(ctx, cudaMalloc(&P.p, n_scalars * 4 + 4));
   RONK_CUDA(ctx, cudaMalloc(&S.p, n_scalars + 4));
   RONK_CUDA(ctx, cudaMemcpyAsync(P.p, points, n_scalars * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -668,11 +617,8 @@ int ronk_msm_combine_buckets_host(ronk_ctx* ctx, const uint8_t* buckets, size_t 
   u32* d_buckets = partial + words;
   u32* d_result = d_buckets + 17;
   if (words) RONK_CUDA(ctx, cudaMemcpyAsync(partial, buckets, words * 4, cudaMemcpyHostToDevice, ctx->stream));
-  {
-    LaunchScope ls(ctx, "msm_finish");
-    msm_finish_kernel<<<1, 16 * MSM_FIN_LANES, 0, ctx->stream>>>(partial, (u32)n_sets, d_buckets, d_result);
-  }
-  RONK_TRY(check_launch(ctx, "msm_finish_kernel"));
+  RONK_TRY(launch(ctx, "msm_finish", msm_finish_kernel, 1, 16 * MSM_FIN_LANES, 0, false, partial, (u32)n_sets, d_buckets,
+                  d_result));
   u32 res;
   RONK_CUDA(ctx, cudaMemcpyAsync(&res, d_result, 4, cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -685,7 +631,7 @@ static int point_op_host(ronk_ctx* ctx, int op, const uint8_t* a, const uint8_t*
   if (!ctx || (n && (!a || !out)) || (n && op == 0 && !b) || (n && op == 2 && !sc))
     return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
-  DevBytes A, B, S, O;
+  DevBuf A, B, S, O;
   RONK_CUDA(ctx, cudaMalloc(&A.p, n * 4));
   RONK_CUDA(ctx, cudaMalloc(&O.p, n * 4));
   RONK_CUDA(ctx, cudaMemcpyAsync(A.p, a, n * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -698,14 +644,8 @@ static int point_op_host(ronk_ctx* ctx, int op, const uint8_t* a, const uint8_t*
     RONK_CUDA(ctx, cudaMemcpyAsync(S.p, sc, n, cudaMemcpyHostToDevice, ctx->stream));
   }
   RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  size_t blocks = (n + 127) / 128;
-  if (blocks > (size_t)ctx->sm_count * 8) blocks = (size_t)ctx->sm_count * 8;
-  {
-    LaunchScope ls(ctx, "point_op");
-    point_op_kernel<<<(int)blocks, 128, 0, ctx->stream>>>(op, (const u32*)A.p, (const u32*)B.p, (const uint8_t*)S.p,
-                                                         (u32*)O.p, n, ctx->d_flag);
-  }
-  RONK_TRY(check_launch(ctx, "point_op_kernel"));
+  RONK_TRY(launch(ctx, "point_op", point_op_kernel, grid_for(ctx, n, 128), 128, 0, false, op, (const u32*)A.p, (const u32*)B.p,
+                  (const uint8_t*)S.p, (u32*)O.p, n, ctx->d_flag));
   RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaMemcpyAsync(out, O.p, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

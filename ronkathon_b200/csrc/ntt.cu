@@ -38,11 +38,7 @@ int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out) {
 template <class F>
 static int build_table(ronk_ctx* ctx, const F& f, u64 w, u64 s, u64** tab, u32 count) {
   RONK_CUDA(ctx, cudaMalloc((void**)tab, (size_t)count * sizeof(u64)));
-  {
-    LaunchScope ls(ctx, "pow_table");
-    pow_table_kernel<F><<<(count + 255) / 256, 256, 0, ctx->stream>>>(f, w, s, *tab, count);
-  }
-  return check_launch(ctx, "pow_table_kernel");
+  return launch(ctx, "pow_table", pow_table_kernel<F>, (count + 255) / 256, 256, 0, false, f, w, s, *tab, count);
 }
 
 static int build_tw2d(ronk_ctx* ctx, const u64* tw1d, u32 log_m, u64* out2d[2]) {
@@ -51,11 +47,7 @@ static int build_tw2d(ronk_ctx* ctx, const u64* tw1d, u32 log_m, u64* out2d[2]) 
   for (int d = 0; d < 2; d++) {
     RONK_CUDA(ctx, cudaMalloc((void**)&out2d[d], (size_t)(words ? words : 2) * sizeof(u64)));
     if (!words) continue;
-    {
-      LaunchScope ls(ctx, "tw2d_gather");
-      tw2d_gather_kernel<<<(words + 255) / 256, 256, 0, ctx->stream>>>(tw1d, log_m, d, out2d[d], words);
-    }
-    RONK_TRY(check_launch(ctx, "tw2d_gather_kernel"));
+    RONK_TRY(launch(ctx, "tw2d_gather", tw2d_gather_kernel, (words + 255) / 256, 256, 0, false, tw1d, log_m, d, out2d[d], words));
   }
   return RONK_OK;
 }
@@ -92,11 +84,10 @@ static int build_plan(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, NttPla
 }
 
 // n-word table of the inter-pass twiddles for one direction and one workspace layout (log2 C2), built on first use.
-// The plan lives in ctx->plans; the table pointer is cached there (mutable through the context).
+// The table pointer is cached in the plan.
 template <class F>
-static int interpass_table(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, bool inverse, u32 log_c2, const u64* tw_lo,
+static int interpass_table(ronk_ctx* ctx, const F& f, NttPlan& pl, bool inverse, u32 log_c2, const u64* tw_lo,
                            const u64* tw_hi, const u64** out) {
-  NttPlan& pl = const_cast<NttPlan&>(pl_c);
   auto& m = pl.tw_full[inverse ? 1 : 0];
   auto it = m.find(log_c2);
   if (it == m.end()) {
@@ -107,12 +98,8 @@ static int interpass_table(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, bool 
       *out = nullptr;  // no memory for the table: the stepped form needs none
       return RONK_OK;
     }
-    {
-      LaunchScope ls(ctx, "interpass_table");
-      interpass_table_kernel<F><<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(
-          f, tw_lo, tw_hi, pl.log_n, pl.log_n1, pl.log_n2, log_c2, pl.log_n1, inverse ? 1 : 0, tab);
-    }
-    RONK_TRY(check_launch(ctx, "interpass_table_kernel"));
+    RONK_TRY(launch(ctx, "interpass_table", interpass_table_kernel<F>, (unsigned)((n + 255) / 256), 256, 0, false, f, tw_lo,
+                    tw_hi, pl.log_n, pl.log_n1, pl.log_n2, log_c2, pl.log_n1, inverse ? 1 : 0, tab));
     it = m.emplace(log_c2, tab).first;
   }
   *out = it->second;
@@ -126,28 +113,10 @@ static int launch_tile_nb(ronk_ctx* ctx, const F& f, const NttTileArgs& A0, u32 
   const size_t smem = ((size_t)1 << A.tile_log) * sizeof(u64) + (size_t)A.tw_words * sizeof(u64) + 16;
   // the attribute is per device: set once per (context, instantiation)
   RONK_TRY(ensure_smem_attr(ctx, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL>, 226 * 1024));
-  {
-    LaunchScope ls(ctx, name);
-    // the early launch helps launch-bound jobs (2^14…2^18) and hurts a 2^24 transform (the waiting CTAs start in
-    // lockstep), so only small jobs take it
-    if (MODE == MODE_PASS2 && ctx->tune.pdl && !ctx->prof && (((u64)tiles << A.tile_log) <= ((u64)1 << 21))) {
-      // pass 2 directly follows its pass 1 on the stream: let it start early (the kernel waits at griddepcontrol.wait)
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(tiles);
-      cfg.blockDim = dim3(NTHR);
-      cfg.dynamicSmemBytes = smem;
-      cfg.stream = ctx->stream;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      RONK_CUDA(ctx, cudaLaunchKernelEx(&cfg, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL>, f, A));
-    } else {
-      ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL><<<tiles, NTHR, smem, ctx->stream>>>(f, A);
-    }
-  }
-  return check_launch(ctx, name);
+  // pass 2 directly follows its pass 1 on the stream and may start early.  That helps launch-bound jobs (2^14…2^18) and
+  // hurts a 2^24 transform (the waiting CTAs start in lockstep), so only small jobs take it
+  const bool pdl = MODE == MODE_PASS2 && ctx->tune.pdl && (((u64)tiles << A.tile_log) <= ((u64)1 << 21));
+  return launch(ctx, name, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL>, tiles, NTHR, smem, pdl, f, A);
 }
 
 // The bounded instantiation exists only where poly_mul needs it: a zero-padded SOURCE enters through
@@ -176,11 +145,7 @@ static int launch12_one(ronk_ctx* ctx, const GoldilocksField& f, const NttTileAr
   if (MODE == MODE_PASS2) A.prefetch_dist = (u32)ctx->tune.pf_dist2 * (u32)ctx->sm_count * (L::NTHR >= 512 ? 1u : 2u);
   const size_t smem = (size_t)L::TILE_SLOTS * 16 + (size_t)L::TW_WORDS * sizeof(u64) + 16;
   RONK_TRY(ensure_smem_attr(ctx, ntt12_kernel<GoldilocksField, MODE, INV, LC, FMUL>, (int)smem));
-  {
-    LaunchScope ls(ctx, name);
-    ntt12_kernel<GoldilocksField, MODE, INV, LC, FMUL><<<tiles, L::NTHR, smem, ctx->stream>>>(f, A);
-  }
-  return check_launch(ctx, name);
+  return launch(ctx, name, ntt12_kernel<GoldilocksField, MODE, INV, LC, FMUL>, tiles, L::NTHR, smem, false, f, A);
 }
 template <int MODE, bool INV>
 static int launch12(ronk_ctx* ctx, const GoldilocksField& f, const NttTileArgs& A, u32 tiles, const char* name) {
@@ -211,22 +176,8 @@ static int launch_tile(ronk_ctx* ctx, const F& f, const NttTileArgs& A, u32 tile
 // ---- transforms as passes of 256-point tiles (ntt3_kernel.cuh): n = 2^24 (three passes) and n = 2^16 (two) -------
 template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int NG, int LI = 0>
 static int launch3_ng(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* name, bool dependent, unsigned tiles) {
-  LaunchScope ls(ctx, name);
-  if (dependent && ctx->tune.ntt3_pdl && !ctx->prof) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(tiles);
-    cfg.blockDim = dim3(N3_THREADS * (2 / NG));
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    RONK_CUDA(ctx, cudaLaunchKernelEx(&cfg, ntt3_kernel<F, PASS, INV, LOGN, BOUNDED, NG, LI>, f, A));
-  } else {
-    ntt3_kernel<F, PASS, INV, LOGN, BOUNDED, NG, LI><<<tiles, N3_THREADS * (2 / NG), 0, ctx->stream>>>(f, A);
-  }
-  return RONK_OK;
+  return launch(ctx, name, ntt3_kernel<F, PASS, INV, LOGN, BOUNDED, NG, LI>, tiles, N3_THREADS * (2 / NG), 0,
+                dependent && ctx->tune.ntt3_pdl, f, A);
 }
 template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int LI = 0>
 static int launch3(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* name, bool dependent) {
@@ -244,22 +195,7 @@ static int launch3(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* nam
 template <class F, bool INV>
 static int launch3c(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* name) {
   const unsigned blocks = (unsigned)((((u64)A.batch << 16) + N3C_THREADS - 1) / N3C_THREADS);
-  LaunchScope ls(ctx, name);
-  if (ctx->tune.ntt3_pdl && !ctx->prof) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(blocks);
-    cfg.blockDim = dim3(N3C_THREADS);
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    RONK_CUDA(ctx, cudaLaunchKernelEx(&cfg, ntt3c_kernel<F, INV>, f, A));
-  } else {
-    ntt3c_kernel<F, INV><<<blocks, N3C_THREADS, 0, ctx->stream>>>(f, A);
-  }
-  return RONK_OK;
+  return launch(ctx, name, ntt3c_kernel<F, INV>, blocks, N3C_THREADS, 0, ctx->tune.ntt3_pdl, f, A);
 }
 
 // first pass of a split transform (ntt3p_kernel): radix 2^LI over the elements n' apart, twiddle, in place
@@ -267,9 +203,7 @@ template <class F, bool INV, int LI>
 static int launch3p(ronk_ctx* ctx, const F& f, const Ntt3Args& A, u32 log_np, u32 log_lo, const char* name) {
   const u64 threads = (u64)A.batch << (log_np - (4 - LI));
   const unsigned blocks = (unsigned)((threads + N3C_THREADS - 1) / N3C_THREADS);
-  LaunchScope ls(ctx, name);
-  ntt3p_kernel<F, INV, LI><<<blocks, N3C_THREADS, 0, ctx->stream>>>(f, A, log_np, log_lo);
-  return RONK_OK;
+  return launch(ctx, name, ntt3p_kernel<F, INV, LI>, blocks, N3C_THREADS, 0, false, f, A, log_np, log_lo);
 }
 
 // one-time tables of the 256-point-tile kernels for one direction: ω_256^x and the 64 Ki-entry ω_65536^(±k·j) [· n^-1]
@@ -283,20 +217,15 @@ static int ntt3_tables(ronk_ctx* ctx, const F& f, NttPlan& pl, int log_n) {
   RONK_TRY(build_table(ctx, f, h_powmod(w, n >> 8, p), 1, &pl.tw256[d], 256));
   RONK_CUDA(ctx, cudaMalloc((void**)&pl.t2[d], 65536 * sizeof(u64)));
   const u64 ninv = INV ? h_powmod(n % p, p - 2, p) : 1;
-  {
-    LaunchScope ls(ctx, "ntt3_t2");
-    ntt3_t2_kernel<F><<<256, 256, 0, ctx->stream>>>(f, h_powmod(w, n >> 16, p), ninv, pl.t2[d]);
-  }
-  return check_launch(ctx, "ntt3_t2_kernel");
+  return launch(ctx, "ntt3_t2", ntt3_t2_kernel<F>, 256, 256, 0, false, f, h_powmod(w, n >> 16, p), ninv, pl.t2[d]);
 }
 
 // Small batches of 2^16-point transforms in ONE launch: a 16-CTA thread-block cluster per transform, the pass-2 → pass-3
 // exchange through distributed shared memory (ntt16c_kernel).  In place, no workspace.  Returns RONK_OK with *done = false
 // when the device refuses the cluster shape (the caller then takes the two-launch path).
 template <class F, bool INV>
-static int run_ntt16_cluster(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, u64* data, const u64* src, const u64* mul, u32 batch,
+static int run_ntt16_cluster(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64* src, const u64* mul, u32 batch,
                              bool* done, u64 mul_mask = ~0ULL) {
-  NttPlan& pl = const_cast<NttPlan&>(pl_c);
   *done = false;
   if (ctx->cluster16_state < 0) return RONK_OK;
   RONK_TRY((ntt3_tables<F, INV>(ctx, f, pl, 16)));
@@ -356,27 +285,27 @@ static int run_ntt16_cluster(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, u64
 // in place in the workspace (its input and output views coincide), pass 3 workspace → data: src is only read, data only
 // written by the last pass, so src == data (in place) and a short data buffer (dst_len words) are both fine.
 // LI > 0: a SPLIT transform n = 2^LI·2^LOGN (2^17 … 2^19 over 2^16, 2^25 / 2^26 over 2^24): `outer` is the n-point plan (its
-// two-level tables feed the first pass), pl_c the 2^LOGN-point plan of the 2^LI·batch sub-transforms; ntt3p_kernel runs
+// two-level tables feed the first pass), pl the 2^LOGN-point plan of the 2^LI·batch sub-transforms; ntt3p_kernel runs
 // first (src → data, in place when they coincide) and the last pass interleaves the sub-transforms' outputs.
 template <class F, bool INV, int LOGN, bool BOUNDED, int LI = 0>
-static int run_ntt3(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, u64* data, const u64* src, const u64* mul, u32 batch,
+static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64* src, const u64* mul, u32 batch,
                     u64 src_len, u64 dst_len, u64 mul_mask = ~0ULL, const NttPlan* outer = nullptr) {
   static_assert(LI == 0 || ((LOGN == 16 || LOGN == 24) && !BOUNDED), "split transforms: over 2^16 or 2^24, unbounded");
-  NttPlan& pl = const_cast<NttPlan&>(pl_c);
   const int d = INV ? 1 : 0;
   const u64 n = (u64)1 << LOGN;
   RONK_TRY((ntt3_tables<F, INV>(ctx, f, pl, LOGN)));
   if (LOGN >= 20 && LOGN <= ctx->tune.ntt3_t1 && !pl.t1[d]) {  // n-word table of the stepped twiddles: 8 MiB (2^20) … 128 MiB (2^24) per direction; no memory: stay stepped
     if (pl.log_n1 != (u32)(LOGN + 1) / 2 || !pl.tw_lo || !pl.tw2) return set_err(ctx, RONK_ECUDA, "internal: unexpected plan shape");
-    if (cudaMalloc((void**)&pl.t1[d], n * sizeof(u64)) == cudaSuccess) {
-      LaunchScope ls(ctx, "ntt3_t1");
-      if (LOGN >= 21) ntt3_t1_kernel<F><<<(unsigned)(n / 256), 256, 0, ctx->stream>>>(f, pl.tw_lo, pl.tw2, INV ? 1 : 0, pl.t1[d], (u32)LOGN);
-      else ntt3_t1_20_kernel<F><<<(unsigned)(n / 256), 256, 0, ctx->stream>>>(f, pl.tw_lo, pl.tw2, INV ? 1 : 0, pl.t1[d]);
-    } else {
+    if (cudaMalloc((void**)&pl.t1[d], n * sizeof(u64)) != cudaSuccess) {
       cudaGetLastError();
       pl.t1[d] = nullptr;
+    } else if (LOGN >= 21) {
+      RONK_TRY(launch(ctx, "ntt3_t1", ntt3_t1_kernel<F>, (unsigned)(n / 256), 256, 0, false, f, pl.tw_lo, pl.tw2, INV ? 1 : 0,
+                      pl.t1[d], (u32)LOGN));
+    } else {
+      RONK_TRY(launch(ctx, "ntt3_t1", ntt3_t1_20_kernel<F>, (unsigned)(n / 256), 256, 0, false, f, pl.tw_lo, pl.tw2, INV ? 1 : 0,
+                      pl.t1[d]));
     }
-    RONK_TRY(check_launch(ctx, "ntt3_t1_kernel"));
   }
   if (LI > 0) {
     if (!outer || !outer->tw_lo || !outer->tw2 || batch > (0x7FFFFFFFu >> (12 + LI))) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
@@ -388,7 +317,6 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, u64* data, c
     P.scale_tw = INV ? f.to_tw(h_powmod((u64)1 << LI, pl.p - 2, pl.p)) : 0;   // 2^-LI: the rest of n^-1 rides on the sub-transforms' tables
     P.batch = batch;
     RONK_TRY((launch3p<F, INV, LI>(ctx, f, P, (u32)LOGN, outer->log_n1, INV ? "intt3_split" : "ntt3_split")));
-    RONK_TRY(check_launch(ctx, "ntt3 split pass"));
     src = data;
     batch <<= LI;
   }
@@ -412,37 +340,31 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, const NttPlan& pl_c, u64* data, c
     // src == data is fine), A2 data → workspace, C workspace → data.  A.tw_hi = ω_n^(1024 y): the plan's 10 / 10 split.
     A.dst = data;
     RONK_TRY((launch3<F, 2, INV, 20, false>(ctx, f, A, INV ? "intt3_a1" : "ntt3_a1", false)));
-    RONK_TRY(check_launch(ctx, "ntt3 pass A1"));
     A.src = data;
     A.dst = (u64*)ctx->ws;
     RONK_TRY((launch3<F, 1, INV, 20, false>(ctx, f, A, INV ? "intt3_a2" : "ntt3_a2", true)));
-    RONK_TRY(check_launch(ctx, "ntt3 pass A2"));
     A.src = (const u64*)ctx->ws;
     A.dst = data;
     A.mul_src = mul;
     A.flags = mul ? NTT_FLAG_MUL : 0;
-    RONK_TRY((launch3c<F, INV>(ctx, f, A, INV ? "intt3_c" : "ntt3_c")));
-    return check_launch(ctx, "ntt3 pass C");
+    return launch3c<F, INV>(ctx, f, A, INV ? "intt3_c" : "ntt3_c");
   } else {
     if constexpr (LOGN >= 21) {
       RONK_TRY((launch3<F, 1, INV, LOGN, BOUNDED>(ctx, f, A, INV ? "intt3_pass1" : "ntt3_pass1", false)));
-      RONK_TRY(check_launch(ctx, "ntt3 pass 1"));
       A.src = (const u64*)ctx->ws;
     }
     RONK_TRY((launch3<F, 2, INV, LOGN, BOUNDED && LOGN == 16>(ctx, f, A, INV ? "intt3_pass2" : "ntt3_pass2", LOGN >= 21)));
-    RONK_TRY(check_launch(ctx, "ntt3 pass 2"));
     A.src = (const u64*)ctx->ws;
     A.dst = data;
     A.mul_src = mul;
     A.flags = mul ? NTT_FLAG_MUL : 0;
-    RONK_TRY((launch3<F, 3, INV, LOGN, BOUNDED, LI>(ctx, f, A, INV ? "intt3_pass3" : "ntt3_pass3", true)));
-    return check_launch(ctx, "ntt3 pass 3");
+    return launch3<F, 3, INV, LOGN, BOUNDED, LI>(ctx, f, A, INV ? "intt3_pass3" : "ntt3_pass3", true);
   }
 }
 
-// the plan of another size for the same (p, g), built on demand (std::map: references to other plans stay valid)
+// the plan of (p, g, 2^log_n), built on first use (std::map: references to other plans stay valid)
 template <class F>
-static int sub_plan(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, const NttPlan** out) {
+static int plan_for(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, NttPlan** out) {
   auto key = std::make_tuple((uint64_t)p, (uint64_t)g, (uint32_t)log_n);
   auto it = ctx->plans.find(key);
   if (it == ctx->plans.end()) {
@@ -458,7 +380,7 @@ static int sub_plan(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, const Nt
 // words and writes data[0, dst_len): the zero padding of poly_mul's operands and the clipping of its
 // result happen inside the load / store phases instead of in separate copy kernels.
 template <class F, bool INV>
-static int run_ntt(ronk_ctx* ctx, const F& f, const NttPlan& pl, u64* data, const u64* mul, u32 batch,
+static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64* mul, u32 batch,
                    const u64* src = nullptr, u64 src_len = NTT_UNBOUNDED, u64 dst_len = NTT_UNBOUNDED,
                    u64 mul_mask = ~0ULL) {
   const u32 log_n = pl.log_n;
@@ -487,8 +409,8 @@ static int run_ntt(ronk_ctx* ctx, const F& f, const NttPlan& pl, u64* data, cons
                                                log_n == 25 || log_n == 26)) {
         // split transforms: a radix-2/4/8 register pass, then 2^16- or 2^24-point tile transforms whose last pass interleaves
         const u32 lsub = log_n >= 25 ? 24u : 16u;
-        const NttPlan* sub = nullptr;
-        RONK_TRY((sub_plan<F>(ctx, f, pl.p, pl.g, lsub, &sub)));
+        NttPlan* sub = nullptr;
+        RONK_TRY(plan_for(ctx, f, pl.p, pl.g, lsub, &sub));
         switch (log_n) {
           case 17: return run_ntt3<F, INV, 16, false, 1>(ctx, f, *sub, data, src, mul, batch, src_len, dst_len, mul_mask, &pl);
           case 18: return run_ntt3<F, INV, 16, false, 2>(ctx, f, *sub, data, src, mul, batch, src_len, dst_len, mul_mask, &pl);
@@ -556,15 +478,10 @@ template <class F>
 static int ntt_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, u64* data, const u64* mul, u32 log_n, u32 batch,
                           int inverse, const u64* src = nullptr, u64 src_len = NTT_UNBOUNDED,
                           u64 dst_len = NTT_UNBOUNDED, u64 mul_mask = ~0ULL) {
-  auto key = std::make_tuple((uint64_t)p, (uint64_t)g, (uint32_t)log_n);
-  auto it = ctx->plans.find(key);
-  if (it == ctx->plans.end()) {
-    NttPlan pl;
-    RONK_TRY(build_plan(ctx, f, p, g, log_n, &pl));
-    it = ctx->plans.emplace(key, pl).first;
-  }
-  return inverse ? run_ntt<F, true>(ctx, f, it->second, data, mul, batch, src, src_len, dst_len, mul_mask)
-                 : run_ntt<F, false>(ctx, f, it->second, data, mul, batch, src, src_len, dst_len, mul_mask);
+  NttPlan* pl = nullptr;
+  RONK_TRY(plan_for(ctx, f, p, g, log_n, &pl));
+  return inverse ? run_ntt<F, true>(ctx, f, *pl, data, mul, batch, src, src_len, dst_len, mul_mask)
+                 : run_ntt<F, false>(ctx, f, *pl, data, mul, batch, src, src_len, dst_len, mul_mask);
 }
 
 // One transform, out of place: dst[0, dst_len) = NTT(src[0, src_len) zero-extended to 2^log_n) [⊙ mul].
@@ -574,13 +491,9 @@ int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len,
   if (!ctx || !src || !dst) return set_err(ctx, RONK_EINVAL, "null argument");
   if (log_n == 0 || log_n > 26 || (p - 1) % ((u64)1 << log_n) != 0)
     return set_err(ctx, RONK_EINVAL, "unsupported transform size");
-  if (is_goldilocks_fast(p, g)) {
-    GoldilocksField f;
+  return with_field(ctx, p, g, inverse != 0, [&](const auto& f) {
     return ntt_with_field(ctx, f, p, g, dst, mul, log_n, 1, inverse, src, src_len, dst_len);
-  }
-  MontField f;
-  RONK_TRY(make_mont_field(ctx, p, g, inverse != 0, &f));
-  return ntt_with_field(ctx, f, p, g, dst, mul, log_n, 1, inverse, src, src_len, dst_len);
+  });
 }
 
 // dst = NTT(src) ⊙ mul (forward), batch transforms, mul an n-word table shared by all of them (index & (n-1)).
@@ -592,13 +505,9 @@ int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst,
     return set_err(ctx, RONK_EINVAL, "unsupported transform size");
   if (batch == 0) return RONK_OK;
   const u64 mask = mul ? (((u64)1 << log_n) - 1) : ~0ULL;
-  if (is_goldilocks_fast(p, g)) {
-    GoldilocksField f;
+  return with_field(ctx, p, g, false, [&](const auto& f) {
     return ntt_with_field(ctx, f, p, g, dst, mul, log_n, batch, 0, src, NTT_UNBOUNDED, NTT_UNBOUNDED, mask);
-  }
-  MontField f;
-  RONK_TRY(make_mont_field(ctx, p, g, false, &f));
-  return ntt_with_field(ctx, f, p, g, dst, mul, log_n, batch, 0, src, NTT_UNBOUNDED, NTT_UNBOUNDED, mask);
+  });
 }
 
 int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n, u32 batch, int inverse) {
@@ -613,13 +522,8 @@ int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n
     if (mul) return ronk_field_mul_u64(ctx, p, (const uint64_t*)data, (const uint64_t*)mul, (uint64_t*)data, batch);
     return RONK_OK;
   }
-  if (is_goldilocks_fast(p, g)) {
-    GoldilocksField f;
-    return ntt_with_field(ctx, f, p, g, data, mul, log_n, batch, inverse);
-  }
-  MontField f;
-  RONK_TRY(make_mont_field(ctx, p, g, inverse != 0, &f));
-  return ntt_with_field(ctx, f, p, g, data, mul, log_n, batch, inverse);
+  return with_field(ctx, p, g, inverse != 0,
+                    [&](const auto& f) { return ntt_with_field(ctx, f, p, g, data, mul, log_n, batch, inverse); });
 }
 
 }  // namespace ronk

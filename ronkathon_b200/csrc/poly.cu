@@ -265,21 +265,11 @@ static int div_linear_with_field(ronk_ctx* ctx, const F& f, const u64* a, size_t
   RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 2 * nchunks * sizeof(u64)));
   u64* S = (u64*)ctx->ws2;
   u64* carry = S + nchunks;
-  {
-    LaunchScope ls(ctx, "div_linear_fold");
-    div_linear_kernel<F, false><<<(u32)nchunks, DL_THR, 0, ctx->stream>>>(f, a, d, z, nullptr, S, scale, nullptr, nullptr);
-  }
-  RONK_TRY(check_launch(ctx, "div_linear_kernel<fold>"));
-  {
-    LaunchScope ls(ctx, "div_linear_carry");
-    div_linear_carry_kernel<F><<<1, 1024, 0, ctx->stream>>>(f, S, (u32)nchunks, z, carry);
-  }
-  RONK_TRY(check_launch(ctx, "div_linear_carry_kernel"));
-  {
-    LaunchScope ls(ctx, "div_linear_apply");
-    div_linear_kernel<F, true><<<(u32)nchunks, DL_THR, 0, ctx->stream>>>(f, a, d, z, carry, nullptr, scale, q, rem);
-  }
-  return check_launch(ctx, "div_linear_kernel<apply>");
+  RONK_TRY(launch(ctx, "div_linear_fold", div_linear_kernel<F, false>, (u32)nchunks, DL_THR, 0, false, f, a, d, z, nullptr, S,
+                  scale, nullptr, nullptr));
+  RONK_TRY(launch(ctx, "div_linear_carry", div_linear_carry_kernel<F>, 1, 1024, 0, false, f, S, (u32)nchunks, z, carry));
+  return launch(ctx, "div_linear_apply", div_linear_kernel<F, true>, (u32)nchunks, DL_THR, 0, false, f, a, d, z, carry, nullptr,
+                scale, q, rem);
 }
 
 // a / (b0 + b1·x): q (d terms, top one 0) and the scalar remainder, all device pointers; q may not alias a.
@@ -292,13 +282,7 @@ static int div_linear_device(ronk_ctx* ctx, u64 p, const u64* a, size_t d, u64 b
   if (b1 == 0) return set_err(ctx, RONK_EINVAL, "divisor is not linear (leading coefficient 0)");
   const u64 b1inv = h_powmod(b1, p - 2, p);
   const u64 z = h_mulmod(b0 ? p - b0 : 0, b1inv, p);
-  if (p == GL_P) {
-    GoldilocksField f;
-    return div_linear_with_field(ctx, f, a, d, z, b1inv, q, rem);
-  }
-  MontField f;
-  RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-  return div_linear_with_field(ctx, f, a, d, z, b1inv, q, rem);
+  return with_field(ctx, p, 0, false, [&](const auto& f) { return div_linear_with_field(ctx, f, a, d, z, b1inv, q, rem); });
 }
 
 // ---- Lagrange interpolation (Reed–Solomon decode, §8f row 2) ------------------------------------
@@ -378,30 +362,10 @@ static int interp_with_field(ronk_ctx* ctx, const F& f, const u64* xs, const u64
   u64* m1 = m0 + (k + 1);
   u64* partial = m1 + (k + 1);
   RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  {
-    LaunchScope ls(ctx, "interp_master");
-    interp_master_kernel<F><<<1, 1024, 0, ctx->stream>>>(f, xs, k, m0, m1);
-  }
-  RONK_TRY(check_launch(ctx, "interp_master_kernel"));
+  RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, xs, k, m0, m1));
   const u64* M = (k & 1) ? m1 : m0;
-  {
-    LaunchScope ls(ctx, "interp_nodes");
-    interp_nodes_kernel<F><<<blocks, 256, 0, ctx->stream>>>(f, M, xs, ys, k, partial, ctx->d_flag);
-  }
-  RONK_TRY(check_launch(ctx, "interp_nodes_kernel"));
-  {
-    LaunchScope ls(ctx, "interp_sum");
-    interp_sum_kernel<F><<<(k + 255) / 256, 256, 0, ctx->stream>>>(f, partial, k, nwarps, out);
-  }
-  return check_launch(ctx, "interp_sum_kernel");
-}
-
-static int grid_for(ronk_ctx* ctx, size_t n, int threads) {
-  size_t blocks = (n + threads - 1) / threads;
-  size_t cap = (size_t)ctx->sm_count * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks == 0) blocks = 1;
-  return (int)blocks;
+  RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, blocks, 256, 0, false, f, M, xs, ys, k, partial, ctx->d_flag));
+  return launch(ctx, "interp_sum", interp_sum_kernel<F>, (k + 255) / 256, 256, 0, false, f, partial, k, nwarps, out);
 }
 
 template <class F>
@@ -414,11 +378,9 @@ static int poly_mul_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u6
   // NTT cost ~ 3·n·log n / 2 multiplies vs da·db for schoolbook
   const double school = (double)da * (double)db;
   const double viantt = 1.5 * (double)((size_t)1 << log_n) * (double)log_n + 4096.0;
-  if (!ntt_ok || school <= viantt) {
-    LaunchScope ls(ctx, "poly_mul_schoolbook");
-    poly_mul_schoolbook_kernel<F><<<grid_for(ctx, L, 128), 128, 0, ctx->stream>>>(f, a, da, b, db, c);
-    return check_launch(ctx, "poly_mul_schoolbook_kernel");
-  }
+  if (!ntt_ok || school <= viantt)
+    return launch(ctx, "poly_mul_schoolbook", poly_mul_schoolbook_kernel<F>, grid_for(ctx, L, 128), 128, 0, false, f, a, da, b,
+                  db, c);
   const size_t n = (size_t)1 << log_n;
   RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 2 * n * sizeof(u64)));
   u64* A = (u64*)ctx->ws2;
@@ -434,13 +396,7 @@ static int poly_mul_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da,
   if (!ctx || !a || !b || !c) return set_err(ctx, RONK_EINVAL, "null argument");
   if (da == 0 || db == 0) return set_err(ctx, RONK_EINVAL, "empty polynomial (D + D2 - 1 underflows)");
   RONK_TRY(validate_modulus(ctx, p));
-  if (is_goldilocks_fast(p, g) || (p == GL_P && g == 0)) {
-    GoldilocksField f;
-    return poly_mul_with_field(ctx, f, p, g, a, da, b, db, c);
-  }
-  MontField f;
-  RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-  return poly_mul_with_field(ctx, f, p, g, a, da, b, db, c);
+  return with_field(ctx, p, g, false, [&](const auto& f) { return poly_mul_with_field(ctx, f, p, g, a, da, b, db, c); });
 }
 
 template <bool SUB>
@@ -448,18 +404,10 @@ static int poly_addsub(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64*
   if (!ctx || (da && (!a || !out)) || (db && !b)) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(validate_modulus(ctx, p));
   if (da == 0) return RONK_OK;
-  const char* name = SUB ? "poly_sub" : "poly_add";
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, name);
-    poly_addsub_kernel<GoldilocksField, SUB><<<grid_for(ctx, da, 256), 256, 0, ctx->stream>>>(f, a, da, b, db, out);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, name);
-    poly_addsub_kernel<MontField, SUB><<<grid_for(ctx, da, 256), 256, 0, ctx->stream>>>(f, a, da, b, db, out);
-  }
-  return check_launch(ctx, name);
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, SUB ? "poly_sub" : "poly_add", poly_addsub_kernel<std::decay_t<decltype(f)>, SUB>, grid_for(ctx, da, 256),
+                  256, 0, false, f, a, da, b, db, out);
+  });
 }
 
 static int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
@@ -467,17 +415,9 @@ static int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const 
   RONK_TRY(validate_modulus(ctx, p));
   if (m == 0) return RONK_OK;
   if (m > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "too many points");
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "poly_eval");
-    poly_eval_kernel<GoldilocksField><<<(u32)m, 256, 0, ctx->stream>>>(f, c, d, xs, out);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, "poly_eval");
-    poly_eval_kernel<MontField><<<(u32)m, 256, 0, ctx->stream>>>(f, c, d, xs, out);
-  }
-  return check_launch(ctx, "poly_eval_kernel");
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "poly_eval", poly_eval_kernel<std::decay_t<decltype(f)>>, (u32)m, 256, 0, false, f, c, d, xs, out);
+  });
 }
 
 // nodes[i] = ω_n^i (plain residues)
@@ -486,22 +426,12 @@ static int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes) {
   if (ronk_root_of_unity(p, g, n, (uint64_t*)&w) != RONK_OK)
     return set_err(ctx, RONK_EINVAL, "n must divide p - 1 (no primitive n-th root of unity)");
   if (n > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "n too large");
-  // plain residues: use the Goldilocks policy's identity to_tw for GL, and for Mont build then
-  // convert back would be wasteful — a dedicated kernel keeps it simple.
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "pow_table");
-    pow_table_kernel<GoldilocksField><<<((u32)n + 255) / 256, 256, 0, ctx->stream>>>(f, w, 1, nodes, (u32)n);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    // to_tw(x) = x·R; passing s = R^-1 yields plain residues
-    const u64 r1 = (u64)((((unsigned __int128)1) << 64) % p);
-    const u64 rinv = h_powmod(r1, p - 2, p);
-    LaunchScope ls(ctx, "pow_table");
-    pow_table_kernel<MontField><<<((u32)n + 255) / 256, 256, 0, ctx->stream>>>(f, w, rinv, nodes, (u32)n);
-  }
-  return check_launch(ctx, "pow_table_kernel");
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    // pow_table_kernel stores to_tw(s·w^i); s = to_tw(1)^-1 (1 for Goldilocks, R^-1 for Montgomery) leaves plain residues
+    const u64 s = h_powmod(f.to_tw(1), p - 2, p);
+    return launch(ctx, "pow_table", pow_table_kernel<std::decay_t<decltype(f)>>, ((u32)n + 255) / 256, 256, 0, false, f, w, s,
+                  nodes, (u32)n);
+  });
 }
 
 static int dft_device(ronk_ctx* ctx, u64 p, u64 g, const u64* in, u64 n, u64* out) {
@@ -566,11 +496,6 @@ static int down(ronk_ctx* ctx, void* h, const u64* d, size_t n) {
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return RONK_OK;
 }
-struct DevBuf {  // frees on scope exit
-  u64* p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-};
-
 int ronk_poly_mul_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* a, size_t da, const uint64_t* b,
                            size_t db, uint64_t* c) {
   ronk::DeviceGuard _dg(ctx);
@@ -621,17 +546,10 @@ int ronk_poly_lagrange_eval_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, cons
   RONK_CUDA(ctx, cudaMalloc((void**)&O.p, sizeof(u64)));
   RONK_TRY(roots_table(ctx, p, g, n, N.p));
   RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "lagrange_eval");
-    lagrange_eval_kernel<GoldilocksField><<<1, 256, 0, ctx->stream>>>(f, C.p, N.p, (u32)n, x, O.p, ctx->d_flag);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, "lagrange_eval");
-    lagrange_eval_kernel<MontField><<<1, 256, 0, ctx->stream>>>(f, C.p, N.p, (u32)n, x, O.p, ctx->d_flag);
-  }
-  RONK_TRY(check_launch(ctx, "lagrange_eval_kernel"));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "lagrange_eval", lagrange_eval_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, C.p, N.p, (u32)n,
+                  x, O.p, ctx->d_flag);
+  }));
   RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_TRY(down(ctx, out, O.p, 1));  // synchronises the stream
   if (*ctx->h_flag)  // mod.rs:386-393: F::ONE.div(x_j - x_m) panics when two nodes coincide (g not of order n)
@@ -652,14 +570,7 @@ int ronk_poly_interpolate_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* xs
   RONK_TRY(up(ctx, &X.p, xs, k));
   RONK_TRY(up(ctx, &Y.p, ys, k));
   RONK_CUDA(ctx, cudaMalloc((void**)&O.p, k * sizeof(u64)));
-  if (p == GL_P) {
-    GoldilocksField f;
-    RONK_TRY(interp_with_field(ctx, f, X.p, Y.p, (u32)k, O.p));
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    RONK_TRY(interp_with_field(ctx, f, X.p, Y.p, (u32)k, O.p));
-  }
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) { return interp_with_field(ctx, f, X.p, Y.p, (u32)k, O.p); }));
   RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_TRY(down(ctx, out, O.p, k));
   if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "interpolation: repeated x coordinate (the reference divides by zero)");
@@ -687,17 +598,10 @@ int ronk_poly_divrem_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, size
   }
   RONK_TRY(up(ctx, &B.p, b, db));
   RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  if (p == GL_P) {
-    GoldilocksField f;
-    LaunchScope ls(ctx, "poly_divrem");
-    poly_divrem_kernel<GoldilocksField><<<1, 256, 0, ctx->stream>>>(f, A.p, (u32)da, B.p, (u32)db, Qd.p, Rd.p, ctx->d_flag);
-  } else {
-    MontField f;
-    RONK_TRY(make_mont_field(ctx, p, 0, false, &f));
-    LaunchScope ls(ctx, "poly_divrem");
-    poly_divrem_kernel<MontField><<<1, 256, 0, ctx->stream>>>(f, A.p, (u32)da, B.p, (u32)db, Qd.p, Rd.p, ctx->d_flag);
-  }
-  RONK_TRY(check_launch(ctx, "poly_divrem_kernel"));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "poly_divrem", poly_divrem_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, A.p, (u32)da, B.p,
+                  (u32)db, Qd.p, Rd.p, ctx->d_flag);
+  }));
   RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaMemcpyAsync(q, Qd.p, da * sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_TRY(down(ctx, r, Rd.p, da));

@@ -8,7 +8,9 @@
 #include <map>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <unordered_set>
+#include <utility>
 #include <vector>
 
 #include "../../include/ronk_b200.h"
@@ -195,6 +197,48 @@ inline int check_launch(ronk_ctx* ctx, const char* what) {
   return RONK_OK;
 }
 
+// One kernel launch on the context's stream, counted and (when profiling) timed under `name`.  pdl: launch with
+// programmatic dependent launch, so the kernel may start before its predecessor on the stream has finished (it waits
+// at griddepcontrol.wait).  Not while profiling: the timing events between the kernels would defeat it.
+template <class... KArgs, class... Args>
+inline int launch(ronk_ctx* ctx, const char* name, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, bool pdl,
+                  Args&&... args) {
+  {
+    LaunchScope ls(ctx, name);
+    if (pdl && !ctx->prof) {
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = grid;
+      cfg.blockDim = block;
+      cfg.dynamicSmemBytes = smem;
+      cfg.stream = ctx->stream;
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      attr[0].val.programmaticStreamSerializationAllowed = 1;
+      cfg.attrs = attr;
+      cfg.numAttrs = 1;
+      RONK_CUDA(ctx, cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
+    } else {
+      kernel<<<grid, block, smem, ctx->stream>>>(std::forward<Args>(args)...);
+    }
+  }
+  return check_launch(ctx, name);
+}
+
+// Grid of a grid-stride kernel over n items: one per thread, at most per_sm CTAs per SM, at least one CTA.
+inline int grid_for(const ronk_ctx* ctx, size_t n, size_t threads, size_t per_sm = 8) {
+  size_t blocks = (n + threads - 1) / threads;
+  const size_t cap = (size_t)ctx->sm_count * per_sm;
+  if (blocks > cap) blocks = cap;
+  if (blocks == 0) blocks = 1;
+  return (int)blocks;
+}
+
+// Device allocation freed on scope exit.
+struct DevBuf {
+  u64* p = nullptr;
+  ~DevBuf() { if (p) cudaFree(p); }
+};
+
 inline int ensure_ws(ronk_ctx* ctx, void** buf, size_t* cap, size_t bytes) {
   if (*cap >= bytes) return RONK_OK;
   if (*buf) {
@@ -212,10 +256,22 @@ inline int ensure_ws(ronk_ctx* ctx, void** buf, size_t* cap, size_t bytes) {
   return RONK_OK;
 }
 
-// Field policy construction (host).
-inline bool is_goldilocks_fast(u64 p, u64 g) { return p == GL_P && g == 7; }
 int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out);  // ntt.cu
 int validate_modulus(ronk_ctx* ctx, u64 p);                                       // field_ops.cu
+
+// Runs fn(f) with the field policy of (p, g) and returns its result.  g is the generator whose roots of unity the call
+// takes from the policy, or 0 when it takes none.  The Goldilocks policy hard-codes ω_16 = 2^156, a power of g = 7, so it
+// serves Goldilocks with g = 7 or 0; every other (p, g) runs on a Montgomery policy built for it.
+template <class Fn>
+inline int with_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, Fn&& fn) {
+  if (p == GL_P && (g == 0 || g == 7)) {
+    GoldilocksField f;
+    return fn(f);
+  }
+  MontField f;
+  RONK_TRY(make_mont_field(ctx, p, g, inverse, &f));
+  return fn(f);
+}
 
 // Internal device-pointer entry points used across translation units.
 int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n, u32 batch, int inverse);
