@@ -187,8 +187,9 @@ int ronk_poly_sub_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t da, c
 /* evaluate — src/polynomial/mod.rs:133-139: out[i] = Σ_j coeffs[j] * xs[i]^j for m points. */
 int ronk_poly_eval_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *coeffs, size_t d, const uint64_t *xs, size_t m, uint64_t *out);
 int ronk_poly_eval_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *coeffs, size_t d, const uint64_t *xs, size_t m, uint64_t *out);
-/* Lagrange-basis evaluate — src/polynomial/mod.rs:382-415 (nodes ω_n^i, barycentric; returns the
- * coefficient itself when x is a node).  Host pointers, n | p-1. */
+/* Lagrange-basis evaluate — src/polynomial/mod.rs:382-415 (nodes ω_n^i, barycentric; returns 0 when x
+ * is a node, because l(x) = 0 multiplies the fold).  Host pointers, n | p-1.  RONK_EINVAL when two
+ * nodes coincide (ω of order below n: the reference divides by zero). */
 int ronk_poly_lagrange_eval_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t n, uint64_t x, uint64_t *out);
 /* quotient_and_remainder / Div / Rem — src/polynomial/mod.rs:170-225, arithmetic.rs:121-146.
  * q and r both have da terms.  Host pointers.  RONK_EINVAL for an all-zero divisor. */

@@ -290,7 +290,12 @@ int orc_lagrange_eval(u64 p, u64 g, const u64 *c, u64 n, u64 x, u64 *out) {
     for (u64 m = 0; m < n; m++)
       if (idx != m) {
         u64 inv;
-        orc_div(p, 1, orc_sub(p, nodes[idx], nodes[m]), &inv);
+        /* :386-393 F::ONE.div(x_j - x_m) panics when ω's order is below n and two nodes coincide */
+        if (orc_div(p, 1, orc_sub(p, nodes[idx], nodes[m]), &inv)) {
+          free(nodes);
+          free(weights);
+          return ORC_EINVAL;
+        }
         wt = orc_mul(p, wt, inv);
       }
     weights[idx] = wt;

@@ -1,4 +1,5 @@
-"""Shared helpers for the -m gpu tests: one Context on torch's current stream, seeded inputs."""
+"""Shared helpers for the -m gpu tests: one Context on torch's current stream, seeded inputs, and exact
+references in Python integers (importable without a GPU)."""
 import numpy as np
 import pytest
 
@@ -77,3 +78,18 @@ def msm_inputs(n, seed_pts=44, seed_sc=45):
     pts = lut[kl[0::2], kl[1::2]]
     sc = oracle.splitmix(17, seed_sc, n).astype(np.uint8)
     return np.ascontiguousarray(pts), sc
+
+
+def lagrange_closed_form(p, g, c, x):
+    """L(x) = (x^n - 1)/n · Σ_j c_j ω^j / (x - ω^j) with Python ints — the barycentric form on the roots of unity,
+    whose weights are ω^j/n.  At a node the reference's fold is multiplied by l(x) = 0, so the value is 0."""
+    n = len(c)
+    w = pow(g, (p - 1) // n, p)
+    xn1 = (pow(x, n, p) - 1) % p
+    if xn1 == 0:
+        return 0
+    acc, wj = 0, 1
+    for cj in c:
+        acc = (acc + int(cj) * wj * pow((x - wj) % p, -1, p)) % p
+        wj = wj * w % p
+    return xn1 * pow(n, -1, p) * acc % p

@@ -294,3 +294,30 @@ def test_extended_curve_has_102_squared_points_and_exponent_102():
 
     for p in sample:
         assert oracle.on_curve(p) and smul(p, 102) == oracle.INF
+
+
+def test_lagrange_eval_panics_on_a_repeated_node_and_matches_the_closed_form():
+    """The oracle's Lagrange evaluate (polynomial/mod.rs:382-415) panics where the reference divides by zero: GL with
+    g = 49 has ω_2 = 49^((p-1)/2) = 1, so both nodes are 1, and g = 7^5 repeats nodes whenever 5 | n.  Where the nodes
+    are distinct it equals the closed form
+    (x^n - 1)/n · Σ_j c_j ω^j / (x - ω^j), which the GPU tests use as the reference above n = 256, and 0 at a node."""
+    from gpu_util import BABYBEAR, PBIG, lagrange_closed_form
+    with pytest.raises(oracle.OraclePanic):
+        oracle.lagrange_eval(GL, [3, 4], 12345, g=49)
+    for p, g in ((101, 2), (GL, 7), (BABYBEAR, 31), (PBIG, 3), (GL, pow(7, 5, GL))):
+        for n in (1, 2, 3, 4, 5, 8, 10, 16, 17, 20, 32, 64):
+            if (p - 1) % n:
+                continue
+            c = oracle.splitmix(p, 400 + n, n)
+            c[-1] = p - 1
+            w = pow(g, (p - 1) // n, p)
+            distinct = len({pow(w, i, p) for i in range(n)}) == n       # g = 7^5 gives ω of order n/5 when 5 | n
+            for x in (0, 1, g, p - 1, w, pow(w, n - 1, p), int(oracle.splitmix(p, 500 + n, 1)[0])):
+                if not distinct:
+                    with pytest.raises(oracle.OraclePanic):
+                        oracle.lagrange_eval(p, c, x, g=g)
+                    continue
+                exp = oracle.lagrange_eval(p, c, x, g=g)
+                assert lagrange_closed_form(p, g, c, x) == exp, (p, n, x)
+                if pow(x, n, p) == 1:
+                    assert exp == 0, (p, n, x)
