@@ -72,6 +72,8 @@ extern "C" {
   pub fn ronk_poly_eval_u64_host(ctx: *mut ronk_ctx, p: u64, coeffs: *const u64, d: usize, xs: *const u64, m: usize, out: *mut u64) -> c_int;
   pub fn ronk_poly_lagrange_eval_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, n: usize, x: u64, out: *mut u64) -> c_int;
   pub fn ronk_poly_divrem_u64_host(ctx: *mut ronk_ctx, p: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;
+  /// `quotient_and_remainder` on device pointers; Newton iteration on the transforms when the divisor's top word is nonzero.
+  pub fn ronk_poly_divrem_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;
   /// Lagrange interpolation = `Message::decode` on the first K coordinates (src/codes/reed_solomon.rs:55-107); host pointers.
   pub fn ronk_poly_interpolate_u64_host(ctx: *mut ronk_ctx, p: u64, xs: *const u64, ys: *const u64, k: usize, out: *mut u64) -> c_int;
   /// Division by b0 + b1·x (the divisor `kzg::open` builds, src/kzg/setup.rs:72-75) as a device-wide scan; device pointers.

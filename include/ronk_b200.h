@@ -194,6 +194,16 @@ int ronk_poly_lagrange_eval_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, cons
 /* quotient_and_remainder / Div / Rem — src/polynomial/mod.rs:170-225, arithmetic.rs:121-146.
  * q and r both have da terms.  Host pointers.  RONK_EINVAL for an all-zero divisor. */
 int ronk_poly_divrem_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *q, uint64_t *r);
+/* quotient_and_remainder / Div / Rem — src/polynomial/mod.rs:170-225, arithmetic.rs:121-146, on DEVICE pointers.
+ * q and r both have da terms (the reference's zero-padded arrays), exactly what ronk_poly_divrem_u64_host returns,
+ * including RONK_EINVAL where the reference panics.  q and r must not alias a, b or each other.  Synchronous: the
+ * host reads b[db-1] to choose a path.  A divisor with a zero top word keeps the literal long division (the
+ * reference's partly reduced remainder and its panics).  Otherwise the division is Euclidean: a linear divisor takes
+ * the scan of ronk_poly_div_linear_u64, and with g != 0 a generator of F_p* (as in ronk_poly_mul_u64) and every
+ * transform of about 2(da - db + 1) and db - 1 points a power of two dividing p - 1 and ≤ 2^26, it runs as Newton
+ * iteration on the transforms (a fixed number of transforms instead of O(da·(da - db)) sequential steps).  g == 0,
+ * or a prime with too few 2-power roots of unity (p = 101, 17, 127), keeps the literal kernel.  Residues canonical. */
+int ronk_poly_divrem_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *q, uint64_t *r);
 /* Division by a linear factor b0 + b1*x — the divisor kzg::open builds (src/kzg/setup.rs:72-75,
  * [-z, 1]) fed to Polynomial::div (src/polynomial/mod.rs:170-225, arithmetic.rs:121-146) — as a
  * device-wide scan.  Device pointers: a (d terms), q (d terms, q[d-1] = 0 like the reference's

@@ -285,6 +285,57 @@ static int div_linear_device(ronk_ctx* ctx, u64 p, const u64* a, size_t d, u64 b
   return with_field(ctx, p, 0, false, [&](const auto& f) { return div_linear_with_field(ctx, f, a, d, z, b1inv, q, rem); });
 }
 
+// The literal long division (poly_divrem_kernel) on device buffers; the panic flag lands in ctx->h_flag[0] once the
+// stream has been synchronised.
+static int divrem_literal(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, u64* q, u64* r) {
+  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "poly_divrem", poly_divrem_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, a, (u32)da, b,
+                  (u32)db, q, r, ctx->d_flag);
+  }));
+  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  return RONK_OK;
+}
+
+static bool overlaps(const u64* x, size_t nx, const u64* y, size_t ny) { return nx && ny && x < y + ny && y < x + nx; }
+
+// quotient_and_remainder (mod.rs:170-225) on device pointers, q and r of da words.  The host reads b[db-1] to choose:
+// a zero top word keeps the reference's quirks (literal kernel); otherwise the division is Euclidean and goes to the
+// cheapest exact path — nothing to do for da < db, the scan for a linear divisor, Newton iteration on the transforms
+// when every transform size divides p - 1, else the literal kernel.
+static int divrem_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64* q, u64* r) {
+  if (!ctx || (da && (!a || !q || !r)) || (db && !b)) return set_err(ctx, RONK_EINVAL, "null argument");
+  RONK_TRY(validate_modulus(ctx, p));
+  if (g >= p) return set_err(ctx, RONK_EINVAL, "generator out of range");
+  if (da > 0x7FFFFFF0ULL || db > 0x7FFFFFF0ULL) return set_err(ctx, RONK_EUNSUPPORTED, "polynomial too long");
+  if (da == 0) return RONK_OK;
+  if (overlaps(q, da, a, da) || overlaps(q, da, b, db) || overlaps(r, da, a, da) || overlaps(r, da, b, db) ||
+      overlaps(q, da, r, da))
+    return set_err(ctx, RONK_EINVAL, "q and r may not alias a, b or each other");
+  u64 lo = 0, top = 0;  // b[0] (linear divisors only) and b[db-1]; an empty divisor counts as zero
+  if (db) {
+    RONK_CUDA(ctx, cudaMemcpyAsync(&top, b + db - 1, sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
+    if (db == 2) RONK_CUDA(ctx, cudaMemcpyAsync(&lo, b, sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
+    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  if (top != 0 && da < db) {  // the reference's loop never runs
+    RONK_CUDA(ctx, cudaMemsetAsync(q, 0, da * sizeof(u64), ctx->stream));
+    RONK_CUDA(ctx, cudaMemcpyAsync(r, a, da * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
+  } else if (top != 0 && db == 2 && top < p && lo < p) {  // as ronk_poly_divrem_u64_host
+    RONK_CUDA(ctx, cudaMemsetAsync(r, 0, da * sizeof(u64), ctx->stream));
+    RONK_TRY(div_linear_device(ctx, p, a, da, lo, top, q, r));
+  } else if (top != 0 && divrem_newton_fits(p, g, da, db)) {
+    RONK_TRY(divrem_newton_device(ctx, p, g, a, da, b, db, top, q, r));
+  } else {
+    RONK_TRY(divrem_literal(ctx, p, a, da, b, db, q, r));
+    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on this divisor");
+    return RONK_OK;
+  }
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return RONK_OK;
+}
+
 // ---- Lagrange interpolation (Reed–Solomon decode, §8f row 2) ------------------------------------
 // Message::decode (codes/reed_solomon.rs:55-107) interpolates the first K coordinates:
 //   data[i] = Σ_j y_j · (-1)^i e_{K-1-i}(x \ x_j) / Π_{k≠j}(x_k - x_j)
@@ -485,6 +536,12 @@ int ronk_poly_div_linear_u64(ronk_ctx* ctx, uint64_t p, const uint64_t* a, size_
   return div_linear_device(ctx, p, (const u64*)a, d, b0, b1, (u64*)q, (u64*)rem);
 }
 
+int ronk_poly_divrem_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* a, size_t da, const uint64_t* b, size_t db,
+                         uint64_t* q, uint64_t* r) {
+  ronk::DeviceGuard _dg(ctx);
+  return divrem_device(ctx, p, g, (const u64*)a, da, (const u64*)b, db, (u64*)q, (u64*)r);
+}
+
 // ---- host-pointer variants ---------------------------------------------------------------------
 static int up(ronk_ctx* ctx, u64** d, const void* h, size_t n) {
   RONK_CUDA(ctx, cudaMalloc((void**)d, (n ? n : 1) * sizeof(u64)));
@@ -597,12 +654,7 @@ int ronk_poly_divrem_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, size
     return down(ctx, r, Rd.p, da);
   }
   RONK_TRY(up(ctx, &B.p, b, db));
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
-    return launch(ctx, "poly_divrem", poly_divrem_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, A.p, (u32)da, B.p,
-                  (u32)db, Qd.p, Rd.p, ctx->d_flag);
-  }));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  RONK_TRY(divrem_literal(ctx, p, A.p, da, B.p, db, Qd.p, Rd.p));
   RONK_CUDA(ctx, cudaMemcpyAsync(q, Qd.p, da * sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_TRY(down(ctx, r, Rd.p, da));
   if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on this divisor");

@@ -1,0 +1,155 @@
+// poly_div.cu — quotient_and_remainder (src/polynomial/mod.rs:170-225, Div/Rem arithmetic.rs:121-146) for a divisor
+// with a nonzero top word, by power-series inversion (Newton iteration) on the transform kernels.  With L = da - db + 1
+// and rev_n(x) the first n words of x reversed:
+//   (1) ar = rev(a)[0, L), hr = rev(b) truncated to min(db, L) words;
+//   (2) inv = hr^-1 mod x^L by doubling: g_1 = b[db-1]^-1, g_2t = g_t·(2 - hr·g_t) mod x^2t, on transforms of 4t points;
+//   (3) rev(q) = ar·inv mod x^L, reversed into q[0, L);
+//   (4) r = a - b·q on its first db - 1 words (r has degree < db - 1): from the low db - 1 words of b and q when the
+//       quotient is that long, else with a, b, q taken mod x^N - 1 for an N ≥ db - 1 (the cyclic difference is r itself).
+// The cost is a fixed number of transforms of about 2L points; the literal kernel (poly.cu) is quadratic.
+// ronk_poly_divrem_u64 (poly.cu) chooses this path; it owns the checks and the quirky divisors.
+#include <algorithm>
+
+#include "ronk_internal.h"
+
+namespace ronk {
+
+// dst[i] = i < n ? src[last - i] : 0, i < dst_len: reverses, truncates and zero-fills in one pass
+__global__ void divrem_reverse_kernel(const u64* __restrict__ src, size_t last, size_t n, u64* __restrict__ dst,
+                                      size_t dst_len) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dst_len; i += stride)
+    dst[i] = (i < n) ? src[last - i] : 0ULL;
+}
+
+// One Newton step point-wise in the transform domain: G[k] ← G[k]·(2 - H[k]·G[k])
+template <class F>
+__global__ void divrem_newton_step_kernel(const F f, u64* __restrict__ G, const u64* __restrict__ H, size_t n) {
+  const u64 two = 2 % f.modulus();
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < n; k += stride) {
+    const u64 g = G[k];
+    G[k] = f.mul(g, f.sub(two, f.mul(H[k], g)));
+  }
+}
+
+// dst[i] = Σ_j src[i + j·n] (the residue mod x^n - 1), i < dst_len ≤ n
+template <class F>
+__global__ void divrem_fold_kernel(const F f, const u64* __restrict__ src, size_t len, size_t n, u64* __restrict__ dst,
+                                   size_t dst_len) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dst_len; i += stride) {
+    u64 acc = 0;
+    for (size_t j = i; j < len; j += n) acc = f.add(acc, src[j]);
+    dst[i] = acc;
+  }
+}
+
+static u32 log2_ceil(size_t v) {  // v ≤ 2^63
+  u32 k = 0;
+  while (k < 63 && ((size_t)1 << k) < v) k++;
+  return k;
+}
+
+// Transform sizes (log2) of the plan: the quotient product (also the largest Newton step) and the remainder product.
+// The remainder needs only b·q mod x^(db-1).  A quotient at least that long is cut to its low db - 1 words, like b,
+// and the product runs without wrap (2(db-1) - 1 points); a shorter one keeps every word and the product is taken mod
+// x^N - 1 with N ≥ db - 1, folding the operands longer than N (dividend, and b when db - 1 = N).
+static void divrem_newton_sizes(size_t da, size_t db, u32* log_q, u32* log_r) {
+  const size_t L = da - db + 1, rw = db - 1;  // L ≥ 1; rw = 0 (a constant divisor): no remainder product
+  *log_q = std::max<u32>(1, log2_ceil(2 * L - 1));
+  *log_r = rw == 0 ? 1 : std::max<u32>(1, L >= rw ? log2_ceil(2 * rw - 1) : log2_ceil(rw));
+}
+
+bool divrem_newton_fits(u64 p, u64 g, size_t da, size_t db) {
+  if (g == 0 || da < db || db == 0) return false;
+  u32 lq, lr;
+  divrem_newton_sizes(da, db, &lq, &lr);
+  const u32 lmax = std::max(lq, lr);
+  return lmax <= 26 && (p - 1) % ((u64)1 << lmax) == 0;
+}
+
+template <class F>
+static int fold(ronk_ctx* ctx, const F& f, const u64* src, size_t len, size_t n, u64* dst, size_t dst_len) {
+  return launch(ctx, "divrem_fold", divrem_fold_kernel<F>, grid_for(ctx, dst_len, 256), 256, 0, false, f, src, len, n, dst,
+                dst_len);
+}
+
+static int reverse(ronk_ctx* ctx, const u64* src, size_t last, size_t n, u64* dst, size_t dst_len) {
+  return launch(ctx, "divrem_reverse", divrem_reverse_kernel, grid_for(ctx, dst_len, 256), 256, 0, false, src, last, n, dst,
+                dst_len);
+}
+
+template <class F>
+static int divrem_newton_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db,
+                                    u64 top, u64* q, u64* r) {
+  const size_t L = da - db + 1, hl = std::min(db, L);
+  u32 lq, lr;
+  divrem_newton_sizes(da, db, &lq, &lr);
+  const size_t nq = (size_t)1 << lq, nr = (size_t)1 << lr, nx = std::max(nq, nr);
+  // own scratch (the transforms use ctx->ws, poly_mul ctx->ws2): X, Y transform buffers | G = inv | AR | HR
+  RONK_TRY(ensure_ws(ctx, &ctx->ws3, &ctx->ws3_bytes, (2 * nx + 2 * L + hl) * sizeof(u64)));
+  u64* X = (u64*)ctx->ws3;
+  u64* Y = X + nx;
+  u64* G = Y + nx;
+  u64* AR = G + L;
+  u64* HR = AR + L;
+  RONK_TRY(reverse(ctx, a, da - 1, L, AR, L));
+  RONK_TRY(reverse(ctx, b, db - 1, hl, HR, hl));
+  // g_1 = b[db-1]^-1 (pageable source: the copy is staged before cudaMemcpyAsync returns)
+  const u64 g1 = h_powmod(top, p - 2, p);
+  RONK_CUDA(ctx, cudaMemcpyAsync(G, &g1, sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
+  for (size_t t = 1; t < L; t *= 2) {
+    // g_t·(2 - hr·g_t) has degree < 4t - 2: the 4t-point cyclic product is exact; keep its first m words
+    const size_t m = std::min(2 * t, L);
+    const u32 ln = log2_ceil(4 * t);
+    RONK_TRY(ntt_device_bounded(ctx, p, g, HR, std::min(hl, m), Y, (u64)1 << ln, nullptr, ln, 0));  // Ĥ of hr mod x^m
+    RONK_TRY(ntt_device_bounded(ctx, p, g, G, t, X, (u64)1 << ln, nullptr, ln, 0));                 // Ĝ of g_t
+    RONK_TRY(launch(ctx, "divrem_newton_step", divrem_newton_step_kernel<F>, grid_for(ctx, (size_t)1 << ln, 256), 256, 0, false,
+                    f, X, (const u64*)Y, (size_t)1 << ln));
+    RONK_TRY(ntt_device_bounded(ctx, p, g, X, (u64)1 << ln, G, m, nullptr, ln, 1));  // g_2t mod x^m
+  }
+  // rev(q) = ar·inv mod x^L (nq ≥ 2L - 1: no wrap into the low L words), into AR, then reversed into q
+  RONK_TRY(ntt_device_bounded(ctx, p, g, AR, L, X, nq, nullptr, lq, 0));
+  RONK_TRY(ntt_device_bounded(ctx, p, g, G, L, Y, nq, X, lq, 0));
+  RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nq, AR, L, nullptr, lq, 1));
+  RONK_TRY(reverse(ctx, AR, L - 1, L, q, da));
+  const size_t rw = db - 1;  // remainder words
+  if (rw == 0) {
+    RONK_CUDA(ctx, cudaMemsetAsync(r, 0, da * sizeof(u64), ctx->stream));
+    return RONK_OK;
+  }
+  const u64* A = a;
+  if (L >= rw) {  // low product: (b mod x^rw)·(q mod x^rw), nr ≥ 2·rw - 1
+    RONK_TRY(ntt_device_bounded(ctx, p, g, b, rw, X, nr, nullptr, lr, 0));
+    RONK_TRY(ntt_device_bounded(ctx, p, g, q, rw, Y, nr, X, lr, 0));
+    RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nr, Y, rw, nullptr, lr, 1));
+  } else {  // b·q mod x^nr - 1, nr ≥ rw > L (q needs no fold; da < 2·rw, so every fold adds at most two terms)
+    if (db > nr) {
+      RONK_TRY(fold(ctx, f, b, db, nr, X, nr));
+      RONK_TRY(ntt_device_bounded(ctx, p, g, X, nr, X, nr, nullptr, lr, 0));
+    } else {
+      RONK_TRY(ntt_device_bounded(ctx, p, g, b, db, X, nr, nullptr, lr, 0));
+    }
+    RONK_TRY(ntt_device_bounded(ctx, p, g, q, L, Y, nr, X, lr, 0));
+    RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nr, Y, rw, nullptr, lr, 1));
+    if (da > nr) {
+      RONK_TRY(fold(ctx, f, a, da, nr, X, rw));
+      A = X;
+    }
+  }
+  RONK_TRY(ronk_poly_sub_u64(ctx, p, (const uint64_t*)A, rw, (const uint64_t*)Y, rw, (uint64_t*)r));
+  if (da > rw) RONK_CUDA(ctx, cudaMemsetAsync(r + rw, 0, (da - rw) * sizeof(u64), ctx->stream));
+  return RONK_OK;
+}
+
+// a / b with b[db-1] = top != 0 and divrem_newton_fits(p, g, da, db); q and r have da words.  Arguments are checked by
+// the caller.  Stream-ordered; the caller synchronises.
+int divrem_newton_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64 top, u64* q,
+                         u64* r) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return divrem_newton_with_field(ctx, f, p, g, a, da, b, db, top, q, r);
+  });
+}
+
+}  // namespace ronk

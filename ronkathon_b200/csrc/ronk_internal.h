@@ -95,6 +95,8 @@ struct ronk_ctx {
   size_t ws_bytes = 0;
   void* ws2 = nullptr;  // second scratch buffer (poly_mul)
   size_t ws2_bytes = 0;
+  void* ws3 = nullptr;  // third scratch buffer (polynomial division by Newton iteration, which calls the transforms)
+  size_t ws3_bytes = 0;
   // two-slot host pipeline (ronk_ntt_u64_host_submit / _wait)
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   static constexpr int kSlots = 3;
@@ -278,5 +280,8 @@ int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n
 int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst, const u64* mul, u32 log_n, u32 batch);
 int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len, u64* dst, u64 dst_len, const u64* mul,
                        u32 log_n, int inverse);
+bool divrem_newton_fits(u64 p, u64 g, size_t da, size_t db);  // poly_div.cu
+int divrem_newton_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64 top, u64* q,
+                         u64* r);
 
 }  // namespace ronk

@@ -50,6 +50,17 @@ def poly_mul(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
     return out
 
 
+def poly_divrem(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
+    """Polynomial::quotient_and_remainder — returns new tensors (q, r), each with len(a) coefficients (zero-padded
+    like the reference's arrays).  Synchronous; raises RonkPanic where the reference panics."""
+    import torch
+    _check_u64(a); _check_u64(b)
+    q = torch.empty_like(a)
+    r = torch.empty_like(a)
+    ctx.call("ronk_poly_divrem_u64", p, g, _lib._ptr(a), a.numel(), _lib._ptr(b), b.numel(), _lib._ptr(q), _lib._ptr(r))
+    return q, r
+
+
 def poly_eval(ctx: Context, coeffs, xs, p: int = GOLDILOCKS):
     import torch
     _check_u64(coeffs); _check_u64(xs)
