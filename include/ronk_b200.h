@@ -15,7 +15,9 @@
  *    cross-checks run through).  p = 2 is not supported (RONK_EUNSUPPORTED).
  *  - Pointers without a `_host` suffix in the function name are DEVICE pointers on the context's
  *    device; work is enqueued on the context's stream and is asynchronous unless stated.
- *    `_host` variants take host pointers, copy in, run, copy out and synchronise.
+ *    `_host` variants take host pointers, copy in, run, copy out and synchronise.  Each context keeps one
+ *    staging buffer for `_host` calls, grown as needed, until ronk_ctx_destroy, like its workspace; a `_host`
+ *    output buffer is written only when the call returns RONK_OK.
  *  - Every function returns 0 (RONK_OK) or an error code; nothing throws, aborts or falls back
  *    to a CPU path.  Where the reference would panic/assert, RONK_EINVAL is returned.
  *  - Curve points (AffinePoint<PlutoExtendedCurve>, src/curve/mod.rs:67-74) are 4 bytes
@@ -192,7 +194,8 @@ int ronk_poly_eval_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *coeffs, s
  * nodes coincide (ω of order below n: the reference divides by zero). */
 int ronk_poly_lagrange_eval_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t n, uint64_t x, uint64_t *out);
 /* quotient_and_remainder / Div / Rem — src/polynomial/mod.rs:170-225, arithmetic.rs:121-146.
- * q and r both have da terms.  Host pointers.  RONK_EINVAL for an all-zero divisor. */
+ * q and r both have da terms.  Host pointers: ronk_poly_divrem_u64 below with g = 0, so a divisor that is not linear
+ * keeps the literal long division.  RONK_EINVAL for an all-zero divisor. */
 int ronk_poly_divrem_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *q, uint64_t *r);
 /* quotient_and_remainder / Div / Rem — src/polynomial/mod.rs:170-225, arithmetic.rs:121-146, on DEVICE pointers.
  * q and r both have da terms (the reference's zero-padded arrays), exactly what ronk_poly_divrem_u64_host returns,
@@ -208,7 +211,7 @@ int ronk_poly_divrem_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *
  * [-z, 1]) fed to Polynomial::div (src/polynomial/mod.rs:170-225, arithmetic.rs:121-146) — as a
  * device-wide scan.  Device pointers: a (d terms), q (d terms, q[d-1] = 0 like the reference's
  * zero-padded quotient), rem (1 word = a(-b0/b1)).  q must not alias a.  RONK_EINVAL for b1 == 0.
- * ronk_poly_divrem_u64_host takes this path by itself when db == 2 and b[1] != 0. */
+ * ronk_poly_divrem_u64[_host] take this path by themselves when db == 2, b[1] != 0 and da >= 2. */
 /* Lagrange interpolation through (xs[i], ys[i]), i < k: the monomial coefficients out[0..k).  This is
  * Message::decode of src/codes/reed_solomon.rs:55-107 applied to the first K coordinates of a
  * codeword (the reference enumerates combinations; the interpolant is unique).  Host pointers,

@@ -112,6 +112,7 @@ int ronk_ctx_destroy(ronk_ctx* ctx) {
   if (ctx->ws) cudaFree(ctx->ws);
   if (ctx->ws2) cudaFree(ctx->ws2);
   if (ctx->ws3) cudaFree(ctx->ws3);
+  if (ctx->stage) cudaFree(ctx->stage);
   if (ctx->msm_ytab) cudaFree(ctx->msm_ytab);
   if (ctx->msm_done) cudaFree(ctx->msm_done);
   if (ctx->msm_coord) cudaFree(ctx->msm_coord);

@@ -141,17 +141,6 @@ int validate_modulus(ronk_ctx* ctx, u64 p) {
   return RONK_OK;
 }
 
-static int reset_flag(ronk_ctx* ctx) {
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  return RONK_OK;
-}
-static int read_flag(ronk_ctx* ctx, int* v) {
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  *v = *ctx->h_flag;
-  return RONK_OK;
-}
-
 template <int OP>
 static int binop(ronk_ctx* ctx, u64 p, const u64* a, const u64* b, u64* out, size_t n, const char* name) {
   if (!ctx || (n && (!a || !b || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
@@ -331,24 +320,15 @@ int ronk_splitmix_fill_u64(ronk_ctx* ctx, uint64_t p, uint64_t seed, uint64_t* o
 }
 
 // ---- host-pointer variants -------------------------------------------------------------------
-static int host_stage(ronk_ctx* ctx, size_t n, u64** da, u64** db, u64** dout) {
-  const size_t bytes = n * sizeof(u64);
-  RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 3 * bytes));
-  *da = (u64*)ctx->ws2;
-  *db = *da + n;
-  *dout = *db + n;
-  return RONK_OK;
-}
-
+// Unlike the device variants, n == 0 returns RONK_OK before the modulus or the op is looked at.
 int ronk_field_binop_u64_host(ronk_ctx* ctx, int op, uint64_t p, const uint64_t* a, const uint64_t* b, uint64_t* out,
                               size_t n) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || (n && (!a || !b || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
-  u64 *da, *db, *dout;
-  RONK_TRY(host_stage(ctx, n, &da, &db, &dout));
-  RONK_CUDA(ctx, cudaMemcpyAsync(da, a, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  RONK_CUDA(ctx, cudaMemcpyAsync(db, b, n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  Staged s[] = {{n * 8, a}, {n * 8, b}, {n * 8, nullptr, out}};
+  RONK_TRY(stage_in(ctx, s));
+  u64 *da = s[0].dev, *db = s[1].dev, *dout = s[2].dev;
   int rc;
   switch (op) {
     case 0: rc = ronk_field_add_u64(ctx, p, da, db, dout, n); break;
@@ -357,39 +337,28 @@ int ronk_field_binop_u64_host(ronk_ctx* ctx, int op, uint64_t p, const uint64_t*
     case 3: rc = ronk_field_div_u64(ctx, p, da, db, dout, n); break;
     default: return set_err(ctx, RONK_EINVAL, "unknown op");
   }
-  if (rc != RONK_OK) return rc;
-  RONK_CUDA(ctx, cudaMemcpyAsync(out, dout, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return RONK_OK;
+  return stage_out(ctx, rc, s);
 }
 
 int ronk_field_unop_u64_host(ronk_ctx* ctx, int op, uint64_t p, const uint64_t* a, uint64_t* out, size_t n) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || (n && (!a || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
-  u64 *da, *db, *dout;
-  RONK_TRY(host_stage(ctx, n, &da, &db, &dout));
-  RONK_CUDA(ctx, cudaMemcpyAsync(da, a, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  int rc = (op == 0)   ? ronk_field_neg_u64(ctx, p, da, dout, n)
-           : (op == 1) ? ronk_field_inv_u64(ctx, p, da, dout, n)
-                       : set_err(ctx, RONK_EINVAL, "unknown op");
-  if (rc != RONK_OK) return rc;
-  RONK_CUDA(ctx, cudaMemcpyAsync(out, dout, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return RONK_OK;
+  Staged s[] = {{n * 8, a}, {n * 8, nullptr, out}};
+  RONK_TRY(stage_in(ctx, s));
+  const int rc = (op == 0)   ? ronk_field_neg_u64(ctx, p, s[0].dev, s[1].dev, n)
+                 : (op == 1) ? ronk_field_inv_u64(ctx, p, s[0].dev, s[1].dev, n)
+                             : set_err(ctx, RONK_EINVAL, "unknown op");
+  return stage_out(ctx, rc, s);
 }
 
 int ronk_field_pow_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, uint64_t e, uint64_t* out, size_t n) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || (n && (!a || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
-  u64 *da, *db, *dout;
-  RONK_TRY(host_stage(ctx, n, &da, &db, &dout));
-  RONK_CUDA(ctx, cudaMemcpyAsync(da, a, n * 8, cudaMemcpyHostToDevice, ctx->stream));
-  RONK_TRY(ronk_field_pow_u64(ctx, p, da, e, dout, n));
-  RONK_CUDA(ctx, cudaMemcpyAsync(out, dout, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return RONK_OK;
+  Staged s[] = {{n * 8, a}, {n * 8, nullptr, out}};
+  RONK_TRY(stage_in(ctx, s));
+  return stage_out(ctx, ronk_field_pow_u64(ctx, p, s[0].dev, e, s[1].dev, n), s);
 }
 
 }  // extern "C"

@@ -594,34 +594,28 @@ int ronk_msm_pluto_ext_buckets(ronk_ctx* ctx, const uint8_t* points, size_t n_po
   return RONK_OK;
 }
 
+// Checked before staging: a null argument, which cannot be uploaded, and the srs length, which the staged call (it
+// passes n_scalars points) no longer sees.
 int ronk_msm_pluto_ext_host(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars,
                             size_t n_scalars, uint8_t out[4]) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || !out || (n_scalars && (!points || !scalars))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n_points < n_scalars) return set_err(ctx, RONK_EINVAL, "srs shorter than coefficients (kzg/setup.rs:53)");
-  DevBuf P, S;
-  RONK_CUDA(ctx, cudaMalloc(&P.p, n_scalars * 4 + 4));
-  RONK_CUDA(ctx, cudaMalloc(&S.p, n_scalars + 4));
-  RONK_CUDA(ctx, cudaMemcpyAsync(P.p, points, n_scalars * 4, cudaMemcpyHostToDevice, ctx->stream));
-  RONK_CUDA(ctx, cudaMemcpyAsync(S.p, scalars, n_scalars, cudaMemcpyHostToDevice, ctx->stream));
-  return ronk_msm_pluto_ext(ctx, (const uint8_t*)P.p, n_scalars, (const uint8_t*)S.p, n_scalars, out);
+  Staged s[] = {{n_scalars * 4, points}, {n_scalars, scalars}};
+  RONK_TRY(stage_in(ctx, s));
+  return stage_out(
+      ctx, ronk_msm_pluto_ext(ctx, (const uint8_t*)s[0].dev, n_scalars, (const uint8_t*)s[1].dev, n_scalars, out), s);
 }
 
 int ronk_msm_combine_buckets_host(ronk_ctx* ctx, const uint8_t* buckets, size_t n_sets, uint8_t out[4]) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || !out || (n_sets && !buckets)) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n_sets > (1u << 20)) return set_err(ctx, RONK_EUNSUPPORTED, "too many bucket sets");
-  const size_t words = n_sets * 17;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, (words + 18) * sizeof(u32)));
-  u32* partial = (u32*)ctx->ws;
-  u32* d_buckets = partial + words;
-  u32* d_result = d_buckets + 17;
-  if (words) RONK_CUDA(ctx, cudaMemcpyAsync(partial, buckets, words * 4, cudaMemcpyHostToDevice, ctx->stream));
-  RONK_TRY(launch(ctx, "msm_finish", msm_finish_kernel, 1, 16 * MSM_FIN_LANES, 0, false, partial, (u32)n_sets, d_buckets,
-                  d_result));
   u32 res;
-  RONK_CUDA(ctx, cudaMemcpyAsync(&res, d_result, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  Staged s[] = {{n_sets * 17 * 4, buckets}, {17 * 4}, {4, nullptr, &res}};  // bucket sets, combined buckets, result
+  RONK_TRY(stage_in(ctx, s));
+  RONK_TRY(stage_out(ctx, launch(ctx, "msm_finish", msm_finish_kernel, 1, 16 * MSM_FIN_LANES, 0, false, (const u32*)s[0].dev,
+                                 (u32)n_sets, (u32*)s[1].dev, (u32*)s[2].dev), s));
   unpack_to_bytes(res, out);
   return RONK_OK;
 }
@@ -631,26 +625,16 @@ static int point_op_host(ronk_ctx* ctx, int op, const uint8_t* a, const uint8_t*
   if (!ctx || (n && (!a || !out)) || (n && op == 0 && !b) || (n && op == 2 && !sc))
     return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
-  DevBuf A, B, S, O;
-  RONK_CUDA(ctx, cudaMalloc(&A.p, n * 4));
-  RONK_CUDA(ctx, cudaMalloc(&O.p, n * 4));
-  RONK_CUDA(ctx, cudaMemcpyAsync(A.p, a, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  if (op == 0) {
-    RONK_CUDA(ctx, cudaMalloc(&B.p, n * 4));
-    RONK_CUDA(ctx, cudaMemcpyAsync(B.p, b, n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  if (op == 2) {
-    RONK_CUDA(ctx, cudaMalloc(&S.p, n));
-    RONK_CUDA(ctx, cudaMemcpyAsync(S.p, sc, n, cudaMemcpyHostToDevice, ctx->stream));
-  }
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  RONK_TRY(launch(ctx, "point_op", point_op_kernel, grid_for(ctx, n, 128), 128, 0, false, op, (const u32*)A.p, (const u32*)B.p,
-                  (const uint8_t*)S.p, (u32*)O.p, n, ctx->d_flag));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaMemcpyAsync(out, O.p, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "Point is not on curve / scalar out of range");
-  return RONK_OK;
+  // a, b (add only), the scalars (smul only), out
+  Staged s[] = {{n * 4, a}, {op == 0 ? n * 4 : 0, b}, {op == 2 ? n : 0, sc}, {n * 4, nullptr, out}};
+  RONK_TRY(stage_in(ctx, s));
+  RONK_TRY(reset_flag(ctx));
+  RONK_TRY(launch(ctx, "point_op", point_op_kernel, grid_for(ctx, n, 128), 128, 0, false, op, (const u32*)s[0].dev,
+                  (const u32*)s[1].dev, (const uint8_t*)s[2].dev, (u32*)s[3].dev, n, ctx->d_flag));
+  int v = 0;
+  RONK_TRY(read_flag(ctx, &v));
+  if (v) return set_err(ctx, RONK_EINVAL, "Point is not on curve / scalar out of range");
+  return stage_out(ctx, RONK_OK, s);
 }
 
 int ronk_point_add_pluto_ext_host(ronk_ctx* ctx, const uint8_t* a, const uint8_t* b, uint8_t* out, size_t n) {

@@ -285,18 +285,6 @@ static int div_linear_device(ronk_ctx* ctx, u64 p, const u64* a, size_t d, u64 b
   return with_field(ctx, p, 0, false, [&](const auto& f) { return div_linear_with_field(ctx, f, a, d, z, b1inv, q, rem); });
 }
 
-// The literal long division (poly_divrem_kernel) on device buffers; the panic flag lands in ctx->h_flag[0] once the
-// stream has been synchronised.
-static int divrem_literal(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, u64* q, u64* r) {
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
-    return launch(ctx, "poly_divrem", poly_divrem_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, a, (u32)da, b,
-                  (u32)db, q, r, ctx->d_flag);
-  }));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  return RONK_OK;
-}
-
 static bool overlaps(const u64* x, size_t nx, const u64* y, size_t ny) { return nx && ny && x < y + ny && y < x + nx; }
 
 // quotient_and_remainder (mod.rs:170-225) on device pointers, q and r of da words.  The host reads b[db-1] to choose:
@@ -321,15 +309,20 @@ static int divrem_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, c
   if (top != 0 && da < db) {  // the reference's loop never runs
     RONK_CUDA(ctx, cudaMemsetAsync(q, 0, da * sizeof(u64), ctx->stream));
     RONK_CUDA(ctx, cudaMemcpyAsync(r, a, da * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
-  } else if (top != 0 && db == 2 && top < p && lo < p) {  // as ronk_poly_divrem_u64_host
+  } else if (top != 0 && db == 2 && top < p && lo < p) {
     RONK_CUDA(ctx, cudaMemsetAsync(r, 0, da * sizeof(u64), ctx->stream));
     RONK_TRY(div_linear_device(ctx, p, a, da, lo, top, q, r));
   } else if (top != 0 && divrem_newton_fits(p, g, da, db)) {
     RONK_TRY(divrem_newton_device(ctx, p, g, a, da, b, db, top, q, r));
-  } else {
-    RONK_TRY(divrem_literal(ctx, p, a, da, b, db, q, r));
-    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on this divisor");
+  } else {  // the literal long division
+    RONK_TRY(reset_flag(ctx));
+    RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+      return launch(ctx, "poly_divrem", poly_divrem_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, a, (u32)da, b,
+                    (u32)db, q, r, ctx->d_flag);
+    }));
+    int v = 0;
+    RONK_TRY(read_flag(ctx, &v));  // synchronises the stream
+    if (v) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on this divisor");
     return RONK_OK;
   }
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -402,21 +395,6 @@ __global__ void interp_sum_kernel(const F f, const u64* __restrict__ partial, u3
   u64 acc = 0;
   for (u32 w = 0; w < nwarps; w++) acc = f.add(acc, partial[(size_t)w * k + i]);
   out[i] = acc;
-}
-
-template <class F>
-static int interp_with_field(ronk_ctx* ctx, const F& f, const u64* xs, const u64* ys, u32 k, u64* out) {
-  const u32 blocks = (k + 255) / 256, nwarps = blocks * 8;
-  const size_t words = 2 * (size_t)(k + 1) + (size_t)nwarps * k;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, words * sizeof(u64)));
-  u64* m0 = (u64*)ctx->ws2;
-  u64* m1 = m0 + (k + 1);
-  u64* partial = m1 + (k + 1);
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
-  RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, xs, k, m0, m1));
-  const u64* M = (k & 1) ? m1 : m0;
-  RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, blocks, 256, 0, false, f, M, xs, ys, k, partial, ctx->d_flag));
-  return launch(ctx, "interp_sum", interp_sum_kernel<F>, (k + 255) / 256, 256, 0, false, f, partial, k, nwarps, out);
 }
 
 template <class F>
@@ -543,49 +521,33 @@ int ronk_poly_divrem_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* 
 }
 
 // ---- host-pointer variants ---------------------------------------------------------------------
-static int up(ronk_ctx* ctx, u64** d, const void* h, size_t n) {
-  RONK_CUDA(ctx, cudaMalloc((void**)d, (n ? n : 1) * sizeof(u64)));
-  if (n) RONK_CUDA(ctx, cudaMemcpyAsync(*d, h, n * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
-  return RONK_OK;
-}
-static int down(ronk_ctx* ctx, void* h, const u64* d, size_t n) {
-  if (n) RONK_CUDA(ctx, cudaMemcpyAsync(h, d, n * sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return RONK_OK;
-}
+// Each stages its arguments, runs the device-pointer function on them and copies the results back.  The device
+// function's checks repeated here are those staging needs first: a null argument cannot be uploaded.
 int ronk_poly_mul_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* a, size_t da, const uint64_t* b,
                            size_t db, uint64_t* c) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || !a || !b || !c) return set_err(ctx, RONK_EINVAL, "null argument");
   if (da == 0 || db == 0) return set_err(ctx, RONK_EINVAL, "empty polynomial (D + D2 - 1 underflows)");
-  DevBuf A, B, C;
-  RONK_TRY(up(ctx, &A.p, a, da));
-  RONK_TRY(up(ctx, &B.p, b, db));
-  RONK_CUDA(ctx, cudaMalloc((void**)&C.p, (da + db - 1) * sizeof(u64)));
-  RONK_TRY(poly_mul_device(ctx, p, g, A.p, da, B.p, db, C.p));
-  return down(ctx, c, C.p, da + db - 1);
+  Staged s[] = {{da * 8, a}, {db * 8, b}, {(da + db - 1) * 8, nullptr, c}};
+  RONK_TRY(stage_in(ctx, s));
+  return stage_out(ctx, poly_mul_device(ctx, p, g, s[0].dev, da, s[1].dev, db, s[2].dev), s);
 }
 
 int ronk_poly_eval_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* coeffs, size_t d, const uint64_t* xs, size_t m,
                             uint64_t* out) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || (m && (!xs || !out)) || (d && !coeffs)) return set_err(ctx, RONK_EINVAL, "null argument");
-  DevBuf C, X, O;
-  RONK_TRY(up(ctx, &C.p, coeffs, d));
-  RONK_TRY(up(ctx, &X.p, xs, m));
-  RONK_CUDA(ctx, cudaMalloc((void**)&O.p, (m ? m : 1) * sizeof(u64)));
-  RONK_TRY(poly_eval_device(ctx, p, C.p, d, X.p, m, O.p));
-  return down(ctx, out, O.p, m);
+  Staged s[] = {{d * 8, coeffs}, {m * 8, xs}, {m * 8, nullptr, out}};
+  RONK_TRY(stage_in(ctx, s));
+  return stage_out(ctx, poly_eval_device(ctx, p, s[0].dev, d, s[1].dev, m, s[2].dev), s);
 }
 
 int ronk_dft_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* in, uint64_t n, uint64_t* out) {
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || !in || !out) return set_err(ctx, RONK_EINVAL, "null argument");
-  DevBuf I, O;
-  RONK_TRY(up(ctx, &I.p, in, n));
-  RONK_CUDA(ctx, cudaMalloc((void**)&O.p, (n ? n : 1) * sizeof(u64)));
-  RONK_TRY(dft_device(ctx, p, g, I.p, n, O.p));
-  return down(ctx, out, O.p, n);
+  Staged s[] = {{n * 8, in}, {n * 8, nullptr, out}};
+  RONK_TRY(stage_in(ctx, s));
+  return stage_out(ctx, dft_device(ctx, p, g, s[0].dev, n, s[1].dev), s);
 }
 
 int ronk_poly_lagrange_eval_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* coeffs, size_t n,
@@ -597,21 +559,19 @@ int ronk_poly_lagrange_eval_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, cons
   if (n == 0 || (p - 1) % n != 0)
     return set_err(ctx, RONK_EINVAL, "n must divide p - 1 (Lagrange::new asserts)");  // mod.rs:361
   if (n > (1u << 20)) return set_err(ctx, RONK_EUNSUPPORTED, "n too large for the O(n²) barycentric form");
-  DevBuf C, N, O;
-  RONK_TRY(up(ctx, &C.p, coeffs, n));
-  RONK_CUDA(ctx, cudaMalloc((void**)&N.p, n * sizeof(u64)));
-  RONK_CUDA(ctx, cudaMalloc((void**)&O.p, sizeof(u64)));
-  RONK_TRY(roots_table(ctx, p, g, n, N.p));
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
+  Staged s[] = {{n * 8, coeffs}, {n * 8}, {8, nullptr, out}};  // coefficients, nodes, result
+  RONK_TRY(stage_in(ctx, s));
+  RONK_TRY(roots_table(ctx, p, g, n, s[1].dev));
+  RONK_TRY(reset_flag(ctx));
   RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
-    return launch(ctx, "lagrange_eval", lagrange_eval_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, C.p, N.p, (u32)n,
-                  x, O.p, ctx->d_flag);
+    return launch(ctx, "lagrange_eval", lagrange_eval_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, s[0].dev,
+                  s[1].dev, (u32)n, x, s[2].dev, ctx->d_flag);
   }));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_TRY(down(ctx, out, O.p, 1));  // synchronises the stream
-  if (*ctx->h_flag)  // mod.rs:386-393: F::ONE.div(x_j - x_m) panics when two nodes coincide (g not of order n)
+  int v = 0;
+  RONK_TRY(read_flag(ctx, &v));
+  if (v)  // mod.rs:386-393: F::ONE.div(x_j - x_m) panics when two nodes coincide (g not of order n)
     return set_err(ctx, RONK_EINVAL, "Lagrange evaluate: repeated node (the reference divides by zero)");
-  return RONK_OK;
+  return stage_out(ctx, RONK_OK, s);
 }
 
 int ronk_poly_interpolate_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* xs, const uint64_t* ys, size_t k,
@@ -623,17 +583,29 @@ int ronk_poly_interpolate_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* xs
   if (k > 8192) return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 nodes (O(K²) interpolation)");
   for (size_t i = 0; i < k; i++)
     if (xs[i] >= p || ys[i] >= p) return set_err(ctx, RONK_EINVAL, "non-canonical residue");
-  DevBuf X, Y, O;
-  RONK_TRY(up(ctx, &X.p, xs, k));
-  RONK_TRY(up(ctx, &Y.p, ys, k));
-  RONK_CUDA(ctx, cudaMalloc((void**)&O.p, k * sizeof(u64)));
-  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) { return interp_with_field(ctx, f, X.p, Y.p, (u32)k, O.p); }));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_TRY(down(ctx, out, O.p, k));
-  if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "interpolation: repeated x coordinate (the reference divides by zero)");
-  return RONK_OK;
+  const u32 blocks = ((u32)k + 255) / 256, nwarps = blocks * 8;
+  // xs, ys, out, then the scratch: the master polynomial's two ping-pong buffers and the per-warp partial sums
+  Staged s[] = {{k * 8, xs}, {k * 8, ys}, {k * 8, nullptr, out}, {(k + 1) * 8}, {(k + 1) * 8}, {nwarps * k * 8}};
+  RONK_TRY(stage_in(ctx, s));
+  const u64 *X = s[0].dev, *Y = s[1].dev;
+  u64 *m0 = s[3].dev, *m1 = s[4].dev, *partial = s[5].dev;
+  RONK_TRY(reset_flag(ctx));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, X, (u32)k, m0, m1));
+    const u64* M = (k & 1) ? m1 : m0;
+    RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, blocks, 256, 0, false, f, M, X, Y, (u32)k, partial,
+                    ctx->d_flag));
+    return launch(ctx, "interp_sum", interp_sum_kernel<F>, blocks, 256, 0, false, f, partial, (u32)k, nwarps, s[2].dev);
+  }));
+  int v = 0;
+  RONK_TRY(read_flag(ctx, &v));
+  if (v) return set_err(ctx, RONK_EINVAL, "interpolation: repeated x coordinate (the reference divides by zero)");
+  return stage_out(ctx, RONK_OK, s);
 }
 
+// ronk_poly_divrem_u64 with g = 0 (no Newton path) on staged copies of a and b.  Its checks up to da == 0 run before
+// staging, in the device function's order, so that an overlong operand is refused before it is copied.
 int ronk_poly_divrem_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, size_t da, const uint64_t* b, size_t db,
                               uint64_t* q, uint64_t* r) {
   ronk::DeviceGuard _dg(ctx);
@@ -641,24 +613,9 @@ int ronk_poly_divrem_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, size
   RONK_TRY(validate_modulus(ctx, p));
   if (da > 0x7FFFFFF0ULL || db > 0x7FFFFFF0ULL) return set_err(ctx, RONK_EUNSUPPORTED, "polynomial too long");
   if (da == 0) return RONK_OK;
-  DevBuf A, B, Qd, Rd;
-  RONK_TRY(up(ctx, &A.p, a, da));
-  RONK_CUDA(ctx, cudaMalloc((void**)&Qd.p, da * sizeof(u64)));
-  RONK_CUDA(ctx, cudaMalloc((void**)&Rd.p, da * sizeof(u64)));
-  if (db == 2 && b[1] != 0 && b[1] < p && b[0] < p) {
-    // linear divisor (the kzg::open case): device-wide scan instead of D sequential steps; the
-    // remainder is the constant a(z), zero-padded to da terms like the reference's array
-    RONK_CUDA(ctx, cudaMemsetAsync(Rd.p, 0, da * sizeof(u64), ctx->stream));
-    RONK_TRY(div_linear_device(ctx, p, A.p, da, b[0], b[1], Qd.p, Rd.p));
-    RONK_CUDA(ctx, cudaMemcpyAsync(q, Qd.p, da * sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
-    return down(ctx, r, Rd.p, da);
-  }
-  RONK_TRY(up(ctx, &B.p, b, db));
-  RONK_TRY(divrem_literal(ctx, p, A.p, da, B.p, db, Qd.p, Rd.p));
-  RONK_CUDA(ctx, cudaMemcpyAsync(q, Qd.p, da * sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
-  RONK_TRY(down(ctx, r, Rd.p, da));
-  if (*ctx->h_flag) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on this divisor");
-  return RONK_OK;
+  Staged s[] = {{da * 8, a}, {db * 8, b}, {da * 8, nullptr, q}, {da * 8, nullptr, r}};
+  RONK_TRY(stage_in(ctx, s));
+  return stage_out(ctx, divrem_device(ctx, p, /*g=*/0, s[0].dev, da, s[1].dev, db, s[2].dev, s[3].dev), s);
 }
 
 }  // extern "C"

@@ -97,6 +97,8 @@ struct ronk_ctx {
   size_t ws2_bytes = 0;
   void* ws3 = nullptr;  // third scratch buffer (polynomial division by Newton iteration, which calls the transforms)
   size_t ws3_bytes = 0;
+  void* stage = nullptr;  // the _host entry points' arguments (stage_in); apart from ws / ws2 / ws3, so they run any path
+  size_t stage_bytes = 0;
   // two-slot host pipeline (ronk_ntt_u64_host_submit / _wait)
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   static constexpr int kSlots = 3;
@@ -235,12 +237,6 @@ inline int grid_for(const ronk_ctx* ctx, size_t n, size_t threads, size_t per_sm
   return (int)blocks;
 }
 
-// Device allocation freed on scope exit.
-struct DevBuf {
-  u64* p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
-};
-
 inline int ensure_ws(ronk_ctx* ctx, void** buf, size_t* cap, size_t bytes) {
   if (*cap >= bytes) return RONK_OK;
   if (*buf) {
@@ -255,6 +251,60 @@ inline int ensure_ws(ronk_ctx* ctx, void** buf, size_t* cap, size_t bytes) {
     return set_err(ctx, RONK_ENOMEM, "workspace allocation failed");
   }
   *cap = bytes;
+  return RONK_OK;
+}
+
+// The device error flag that kernels raise with atomicExch: cleared before a launch, read back (synchronising the
+// stream) after it.
+inline int reset_flag(ronk_ctx* ctx) {
+  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
+  return RONK_OK;
+}
+inline int read_flag(ronk_ctx* ctx, int* v) {
+  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  *v = *ctx->h_flag;
+  return RONK_OK;
+}
+
+// One region of a _host call's arguments in ctx->stage: `bytes` uploaded from `in` before the call when `in` is set,
+// downloaded to `out` after a successful call when `out` is set, scratch when neither is.
+struct Staged {
+  size_t bytes;
+  const void* in = nullptr;
+  void* out = nullptr;
+  u64* dev = nullptr;  // set by stage_in
+};
+
+// Every region starts on a 256-byte boundary, as a cudaMalloc'd buffer would (msm_coord_kernel's vector path needs
+// 16-byte aligned points), and takes at least one block, so that an empty region is still a valid pointer.
+constexpr size_t kStageAlign = 256;
+inline size_t stage_span(size_t bytes) { return (bytes / kStageAlign + 1) * kStageAlign; }
+
+// Carves the regions from ctx->stage, growing it once for all of them before any is handed out (growing frees the
+// old buffer), and enqueues the uploads on ctx->stream.
+template <size_t N>
+inline int stage_in(ronk_ctx* ctx, Staged (&r)[N]) {
+  size_t total = 0;
+  for (const Staged& s : r) total += stage_span(s.bytes);
+  RONK_TRY(ensure_ws(ctx, &ctx->stage, &ctx->stage_bytes, total));
+  char* at = (char*)ctx->stage;
+  for (Staged& s : r) {
+    s.dev = (u64*)at;
+    at += stage_span(s.bytes);
+    if (s.in && s.bytes) RONK_CUDA(ctx, cudaMemcpyAsync(s.dev, s.in, s.bytes, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  return RONK_OK;
+}
+
+// Ends a staged call whose device work returned rc: on RONK_OK copies the outputs back and synchronises; otherwise
+// returns rc and leaves the host outputs unwritten.
+template <size_t N>
+inline int stage_out(ronk_ctx* ctx, int rc, const Staged (&r)[N]) {
+  if (rc != RONK_OK) return rc;
+  for (const Staged& s : r)
+    if (s.out && s.bytes) RONK_CUDA(ctx, cudaMemcpyAsync(s.out, s.dev, s.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return RONK_OK;
 }
 

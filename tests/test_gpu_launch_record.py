@@ -34,12 +34,26 @@ def _poly_mul(da, db, p=GL, g=7):
     return lambda c: ops.poly_mul(c, a, b, p=p, g=g)
 
 
+def _poly_mul_host(da, db):
+    from ronkathon_b200 import _lib
+    a, b = oracle.splitmix(GL, 14, da), oracle.splitmix(GL, 15, db)
+    out = np.empty(da + db - 1, dtype=np.uint64)
+    return lambda c: c.call("ronk_poly_mul_u64_host", GL, 7, _lib._ptr(a), da, _lib._ptr(b), db, _lib._ptr(out))
+
+
 def _binop(name, p):
     import torch
     from ronkathon_b200 import _lib
     a, b = dev(oracle.splitmix(p, 16, 4096)), dev(oracle.splitmix(p - 1, 17, 4096) + 1)
     out = torch.empty_like(a)
     return lambda c: c.call(f"ronk_field_{name}_u64", p, _lib._ptr(a), _lib._ptr(b), _lib._ptr(out), 4096)
+
+
+def _binop_host(op, p):
+    from ronkathon_b200 import _lib
+    a, b = oracle.splitmix(p, 16, 4096), oracle.splitmix(p - 1, 17, 4096) + 1
+    out = np.empty(4096, dtype=np.uint64)
+    return lambda c: c.call("ronk_field_binop_u64_host", op, p, _lib._ptr(a), _lib._ptr(b), _lib._ptr(out), 4096)
 
 
 def _unop(name, p):
@@ -89,6 +103,13 @@ def _dft(p, g):
     return lambda c: c.call("ronk_dft_u64", p, g, _lib._ptr(a), 1024, _lib._ptr(out))
 
 
+def _dft_host(p, g):
+    from ronkathon_b200 import _lib
+    a = oracle.splitmix(p, 24, 1024)
+    out = np.empty_like(a)
+    return lambda c: c.call("ronk_dft_u64_host", p, g, _lib._ptr(a), 1024, _lib._ptr(out))
+
+
 def _lagrange(p, g):
     from ronkathon_b200 import _lib
     coeffs = oracle.splitmix(p, 25, 256)
@@ -134,6 +155,13 @@ def _msm():
     return lambda c: ops.msm(c, P, S)
 
 
+def _msm_host():
+    from ronkathon_b200 import _lib
+    pts, sc = msm_inputs(1 << 16)
+    out = np.empty(4, dtype=np.uint8)
+    return lambda c: c.call("ronk_msm_pluto_ext_host", _lib._ptr(pts), len(sc), _lib._ptr(sc), len(sc), _lib._ptr(out))
+
+
 def _splitmix():
     import torch
     from ronkathon_b200 import ops
@@ -165,7 +193,10 @@ CASES = {
     "poly_mul_2^23x2^23": (lambda: _poly_mul(1 << 23, 1 << 23), _NTT3 + _NTT3 + _INTT3),
     "poly_mul_babybear_ntt": (lambda: _poly_mul(256, 256, p=BABYBEAR, g=BB_G), _POLY_MUL_SINGLE),
     "poly_mul_gl_g0": (lambda: _poly_mul(256, 256, g=0), ["poly_mul_schoolbook"]),
+    "poly_mul_host_schoolbook": (lambda: _poly_mul_host(64, 64), ["poly_mul_schoolbook"]),
+    "poly_mul_host_ntt": (lambda: _poly_mul_host(256, 256), _POLY_MUL_SINGLE),
     "msm": (_msm, ["msm_coord"]),
+    "msm_host": (_msm_host, ["msm_coord"]),
     "splitmix_fill": (_splitmix, ["splitmix_fill"]),
 }
 for _pn, _p, _g in (("gl", GL, 7), ("babybear", BABYBEAR, BB_G)):
@@ -177,7 +208,9 @@ for _pn, _p, _g in (("gl", GL, 7), ("babybear", BABYBEAR, BB_G)):
         f"poly_add_{_pn}": ((lambda p=_p: _poly_addsub("add", p)), ["poly_add"]),
         f"poly_sub_{_pn}": ((lambda p=_p: _poly_addsub("sub", p)), ["poly_sub"]),
         f"poly_eval_{_pn}": ((lambda p=_p: _poly_eval(p)), ["poly_eval"]),
+        f"field_div_host_{_pn}": ((lambda p=_p: _binop_host(3, p)), ["field_div"]),
         f"dft_{_pn}": ((lambda p=_p, g=_g: _dft(p, g)), ["pow_table", "poly_eval"]),
+        f"dft_host_{_pn}": ((lambda p=_p, g=_g: _dft_host(p, g)), ["pow_table", "poly_eval"]),
         f"lagrange_eval_{_pn}": ((lambda p=_p, g=_g: _lagrange(p, g)), ["pow_table", "lagrange_eval"]),
         f"interpolate_{_pn}": ((lambda p=_p: _interpolate(p)), ["interp_master", "interp_nodes", "interp_sum"]),
         f"divrem_linear_{_pn}": ((lambda p=_p: _divrem([5, 1], p)), _DIV_LINEAR),
