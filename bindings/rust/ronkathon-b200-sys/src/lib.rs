@@ -76,6 +76,12 @@ extern "C" {
   pub fn ronk_poly_divrem_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;
   /// Lagrange interpolation = `Message::decode` on the first K coordinates (src/codes/reed_solomon.rs:55-107); host pointers.
   pub fn ronk_poly_interpolate_u64_host(ctx: *mut ronk_ctx, p: u64, xs: *const u64, ys: *const u64, k: usize, out: *mut u64) -> c_int;
+  /// Π (X - xs[i]) on device pointers, k + 1 coefficients; a subproduct tree on the transforms above the crossover.
+  pub fn ronk_poly_from_roots_u64(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, k: usize, out: *mut u64) -> c_int;
+  /// `evaluate` at m points on device pointers (src/shamir/mod.rs:53-58); the same words as `ronk_poly_eval_u64`.
+  pub fn ronk_poly_multieval_u64(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, d: usize, xs: *const u64, m: usize, out: *mut u64) -> c_int;
+  /// Device twin of `ronk_poly_interpolate_u64_host`; synchronous.
+  pub fn ronk_poly_interpolate_u64(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, ys: *const u64, k: usize, out: *mut u64) -> c_int;
   /// Division by b0 + b1·x (the divisor `kzg::open` builds, src/kzg/setup.rs:72-75) as a device-wide scan; device pointers.
   pub fn ronk_poly_div_linear_u64(ctx: *mut ronk_ctx, p: u64, a: *const u64, d: usize, b0: u64, b1: u64, q: *mut u64, rem: *mut u64) -> c_int;
 

@@ -217,6 +217,26 @@ int ronk_poly_divrem_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *
  * codeword (the reference enumerates combinations; the interpolant is unique).  Host pointers,
  * k <= 8192.  RONK_EINVAL for a repeated x (the reference's `/` panics on the zero denominator). */
 int ronk_poly_interpolate_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *xs, const uint64_t *ys, size_t k, uint64_t *out);
+/* Multipoint evaluation and interpolation on a subproduct tree, DEVICE pointers, on the context's stream.
+ * Path rule (as ronk_poly_divrem_u64): the tree runs in O(n log² n) when g != 0 is a generator of F_p*, every transform
+ * of its plan is a power of two dividing p - 1 and ≤ 2^26, and the size reaches a measured crossover (DESIGN.md §3.5);
+ * otherwise the existing kernels run.  Envelope: at most 2^24 points (tree leaves; the largest tree transform has 2^25
+ * points), else RONK_EUNSUPPORTED.  RONK_EINVAL for a null pointer, g >= p, or an output that overlaps an input.
+ * Nothing is written on failure.  Residues canonical. */
+/* Π_{i<k} (X - xs[i]): out has k + 1 coefficients, out[k] = 1 (k = 0: out[0] = 1).  Off the tree: one CTA of k
+ * sequential linear products, at most 8192 roots (RONK_EUNSUPPORTED above); k ≤ 64 is always the tree's shared-memory
+ * kernel alone.  Asynchronous. */
+int ronk_poly_from_roots_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, size_t k, uint64_t *out);
+/* evaluate — src/polynomial/mod.rs:133-139 at m points, as Shamir split evaluates at 1..n (src/shamir/mod.rs:53-58):
+ * out[i] = Σ_j coeffs[j]·xs[i]^j, i < m, the same words as ronk_poly_eval_u64 for every d (including 0) and m; repeated
+ * points are fine.  The tree path also needs d ≤ 2^25 (its root division has transforms of 2·d points); off it,
+ * ronk_poly_eval_u64's kernel runs.  Asynchronous. */
+int ronk_poly_multieval_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t d, const uint64_t *xs, size_t m, uint64_t *out);
+/* Device twin of ronk_poly_interpolate_u64_host (Message::decode, src/codes/reed_solomon.rs:55-107): the unique
+ * interpolant through (xs[i], ys[i]), k coefficients.  Off the tree path it runs the same kernels as the host variant,
+ * capped at 8192 nodes (RONK_EUNSUPPORTED above); the tree takes every k > 8192 it fits.  Synchronous; RONK_EINVAL for a
+ * repeated x (the reference's `/` panics on the zero denominator). */
+int ronk_poly_interpolate_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *ys, size_t k, uint64_t *out);
 int ronk_poly_div_linear_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t d, uint64_t b0, uint64_t b1, uint64_t *q, uint64_t *rem);
 
 /* ---- curve + kzg::commit ------------------------------------------------------------------ */

@@ -68,6 +68,9 @@ SIGNATURES = {
     "ronk_poly_divrem_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp, vp]),
     "ronk_poly_div_linear_u64": (i32, [vp, u64, vp, sz, u64, u64, vp, vp]),
     "ronk_poly_interpolate_u64_host": (i32, [vp, u64, vp, vp, sz, vp]),
+    "ronk_poly_from_roots_u64": (i32, [vp, u64, u64, vp, sz, vp]),
+    "ronk_poly_multieval_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
+    "ronk_poly_interpolate_u64": (i32, [vp, u64, u64, vp, vp, sz, vp]),
     "ronk_point_add_pluto_ext_host": (i32, [vp, vp, vp, vp, sz]),
     "ronk_point_neg_pluto_ext_host": (i32, [vp, vp, vp, sz]),
     "ronk_point_smul_pluto_ext_host": (i32, [vp, vp, vp, vp, sz]),

@@ -61,6 +61,7 @@ int ronk_ctx_create(ronk_ctx** out, int device, void* stream) {
   ctx->tune.msm_coord = env_int("RONK_MSM_COORD", 1);
   ctx->tune.msm_hist = env_int("RONK_MSM_HIST", 1);
   ctx->tune.msm_split = env_int("RONK_MSM_SPLIT", 0);
+  ctx->tune.tree_min = env_int("RONK_TREE_MIN", -1);
   ctx->stream = (cudaStream_t)stream;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return RONK_ECUDA; }
@@ -112,6 +113,7 @@ int ronk_ctx_destroy(ronk_ctx* ctx) {
   if (ctx->ws) cudaFree(ctx->ws);
   if (ctx->ws2) cudaFree(ctx->ws2);
   if (ctx->ws3) cudaFree(ctx->ws3);
+  if (ctx->ws4) cudaFree(ctx->ws4);
   if (ctx->stage) cudaFree(ctx->stage);
   if (ctx->msm_ytab) cudaFree(ctx->msm_ytab);
   if (ctx->msm_done) cudaFree(ctx->msm_done);

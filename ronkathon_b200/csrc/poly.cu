@@ -463,6 +463,99 @@ static int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes) {
   });
 }
 
+// The literal interpolation (interp_* kernels above) through k ≤ 8192 nodes into out; scratch m0 and m1 of k + 1 words,
+// partial of ⌈k/256⌉·8·k words.  Synchronous; RONK_EINVAL for a repeated x, with out written.
+static int interp_literal(ronk_ctx* ctx, u64 p, const u64* X, const u64* Y, size_t k, u64* out, u64* m0, u64* m1,
+                          u64* partial) {
+  const u32 blocks = ((u32)k + 255) / 256, nwarps = blocks * 8;
+  RONK_TRY(reset_flag(ctx));
+  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, X, (u32)k, m0, m1));
+    const u64* M = (k & 1) ? m1 : m0;
+    RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, blocks, 256, 0, false, f, M, X, Y, (u32)k, partial,
+                    ctx->d_flag));
+    return launch(ctx, "interp_sum", interp_sum_kernel<F>, blocks, 256, 0, false, f, partial, (u32)k, nwarps, out);
+  }));
+  int v = 0;
+  RONK_TRY(read_flag(ctx, &v));
+  if (v) return set_err(ctx, RONK_EINVAL, "interpolation: repeated x coordinate (the reference divides by zero)");
+  return RONK_OK;
+}
+constexpr size_t kInterpLiteralMax = 8192;
+
+// ---- subproduct-tree entry points (poly_tree.cu), SURVEY §8f rows 2 and 3 --------------------------------------------
+// The tree runs when g != 0, every transform of its plan divides p - 1 (tree_fits) and the size reaches the crossover,
+// else the existing kernels do.  The crossovers are tools/multipoint_timing.py's on an H100 80GB HBM3 at 400 W (DESIGN.md
+// §5): the smallest power of two from which the tree won at every larger size measured.  RONK_TREE_MIN overrides all three.
+constexpr size_t kFromRootsTreeMin = 128;     // k (0.049 vs 0.050 ms); k ≤ kTreeLeaves is the tree's shared-memory kernel alone
+constexpr size_t kMultievalTreeMin = 32768;   // min(d, m), timed at d = m (1.84 vs 1.96 ms; 2^14: 1.66 vs 0.58)
+constexpr size_t kInterpTreeMin = 2048;       // k (1.13 vs 1.89 ms; 1024: 1.25 vs 0.89); above kInterpLiteralMax always the tree
+
+static size_t tree_min(const ronk_ctx* ctx, size_t measured) {
+  return ctx->tune.tree_min >= 0 ? (size_t)ctx->tune.tree_min : measured;
+}
+
+// Checks shared by the three: RONK_EINVAL for a null pointer or g out of range, RONK_EUNSUPPORTED above 2^24 points.
+static int tree_args(ronk_ctx* ctx, u64 p, u64 g, size_t k, bool null_arg) {
+  if (!ctx || null_arg) return set_err(ctx, RONK_EINVAL, "null argument");
+  RONK_TRY(validate_modulus(ctx, p));
+  if (g >= p) return set_err(ctx, RONK_EINVAL, "generator out of range");
+  if (k > kTreeMaxLeaves) return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^24 points");
+  return RONK_OK;
+}
+
+static int from_roots_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out) {
+  RONK_TRY(tree_args(ctx, p, g, k, !out || (k && !xs)));
+  if (overlaps(out, k + 1, xs, k)) return set_err(ctx, RONK_EINVAL, "out may not overlap xs");
+  if (k == 0) {  // the empty product (pageable source: staged before cudaMemcpyAsync returns)
+    const u64 one = 1;
+    RONK_CUDA(ctx, cudaMemcpyAsync(out, &one, sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
+    return RONK_OK;
+  }
+  if (k <= kTreeLeaves || (tree_fits(p, g, k, 0) && k >= tree_min(ctx, kFromRootsTreeMin)))
+    return tree_from_roots(ctx, p, g, xs, k, out);
+  if (k > kInterpLiteralMax)
+    return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 roots off the tree path (k sequential linear products)");
+  // k linear products in one CTA (interp_master_kernel), ping-ponging between out and k + 1 words of scratch so that
+  // the last one lands in out
+  RONK_TRY(ensure_ws(ctx, &ctx->ws4, &ctx->ws4_bytes, (k + 1) * sizeof(u64)));
+  u64* tmp = (u64*)ctx->ws4;
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "interp_master", interp_master_kernel<std::decay_t<decltype(f)>>, 1, 1024, 0, false, f, xs, (u32)k,
+                  (k & 1) ? tmp : out, (k & 1) ? out : tmp);
+  });
+}
+
+static int multieval_device(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
+  RONK_TRY(tree_args(ctx, p, g, m, (m && (!xs || !out)) || (d && !c)));
+  if (m == 0) return RONK_OK;
+  if (overlaps(out, m, xs, m) || overlaps(out, m, c, d)) return set_err(ctx, RONK_EINVAL, "out may not overlap coeffs or xs");
+  if (d && tree_fits(p, g, m, d) && std::min(d, m) >= tree_min(ctx, kMultievalTreeMin))
+    return tree_multieval(ctx, p, g, c, d, xs, m, out);
+  return poly_eval_device(ctx, p, c, d, xs, m, out);
+}
+
+static int interpolate_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u64* out) {
+  RONK_TRY(tree_args(ctx, p, g, k, k && (!xs || !ys || !out)));
+  if (k == 0) return RONK_OK;
+  if (overlaps(out, k, xs, k) || overlaps(out, k, ys, k)) return set_err(ctx, RONK_EINVAL, "out may not overlap xs or ys");
+  if (tree_fits(p, g, k, k) && (k >= tree_min(ctx, kInterpTreeMin) || k > kInterpLiteralMax))
+    return tree_interpolate(ctx, p, g, xs, ys, k, out);
+  if (k > kInterpLiteralMax)
+    return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 nodes off the tree path (O(K²) interpolation)");
+  // the literal kernels into scratch, so that a repeated x leaves out unwritten
+  const size_t nwarps = (k + 255) / 256 * 8;
+  RONK_TRY(ensure_ws(ctx, &ctx->ws4, &ctx->ws4_bytes, (3 * k + 2 + nwarps * k) * sizeof(u64)));
+  u64* res = (u64*)ctx->ws4;
+  u64* m0 = res + k;
+  u64* m1 = m0 + k + 1;
+  RONK_TRY(interp_literal(ctx, p, xs, ys, k, res, m0, m1, m1 + k + 1));
+  RONK_CUDA(ctx, cudaMemcpyAsync(out, res, k * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return RONK_OK;
+}
+
 static int dft_device(ronk_ctx* ctx, u64 p, u64 g, const u64* in, u64 n, u64* out) {
   if (!ctx || !in || !out) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(validate_modulus(ctx, p));
@@ -583,25 +676,29 @@ int ronk_poly_interpolate_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* xs
   if (k > 8192) return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 nodes (O(K²) interpolation)");
   for (size_t i = 0; i < k; i++)
     if (xs[i] >= p || ys[i] >= p) return set_err(ctx, RONK_EINVAL, "non-canonical residue");
-  const u32 blocks = ((u32)k + 255) / 256, nwarps = blocks * 8;
+  const size_t nwarps = (k + 255) / 256 * 8;
   // xs, ys, out, then the scratch: the master polynomial's two ping-pong buffers and the per-warp partial sums
   Staged s[] = {{k * 8, xs}, {k * 8, ys}, {k * 8, nullptr, out}, {(k + 1) * 8}, {(k + 1) * 8}, {nwarps * k * 8}};
   RONK_TRY(stage_in(ctx, s));
-  const u64 *X = s[0].dev, *Y = s[1].dev;
-  u64 *m0 = s[3].dev, *m1 = s[4].dev, *partial = s[5].dev;
-  RONK_TRY(reset_flag(ctx));
-  RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
-    using F = std::decay_t<decltype(f)>;
-    RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, X, (u32)k, m0, m1));
-    const u64* M = (k & 1) ? m1 : m0;
-    RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, blocks, 256, 0, false, f, M, X, Y, (u32)k, partial,
-                    ctx->d_flag));
-    return launch(ctx, "interp_sum", interp_sum_kernel<F>, blocks, 256, 0, false, f, partial, (u32)k, nwarps, s[2].dev);
-  }));
-  int v = 0;
-  RONK_TRY(read_flag(ctx, &v));
-  if (v) return set_err(ctx, RONK_EINVAL, "interpolation: repeated x coordinate (the reference divides by zero)");
+  RONK_TRY(interp_literal(ctx, p, s[0].dev, s[1].dev, k, s[2].dev, s[3].dev, s[4].dev, s[5].dev));
   return stage_out(ctx, RONK_OK, s);
+}
+
+int ronk_poly_from_roots_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, size_t k, uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  return from_roots_device(ctx, p, g, (const u64*)xs, k, (u64*)out);
+}
+
+int ronk_poly_multieval_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* coeffs, size_t d, const uint64_t* xs,
+                            size_t m, uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  return multieval_device(ctx, p, g, (const u64*)coeffs, d, (const u64*)xs, m, (u64*)out);
+}
+
+int ronk_poly_interpolate_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, const uint64_t* ys, size_t k,
+                              uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  return interpolate_device(ctx, p, g, (const u64*)xs, (const u64*)ys, k, (u64*)out);
 }
 
 // ronk_poly_divrem_u64 with g = 0 (no Newton path) on staged copies of a and b.  Its checks up to da == 0 run before

@@ -80,6 +80,30 @@ static int reverse(ronk_ctx* ctx, const u64* src, size_t last, size_t n, u64* ds
                 dst_len);
 }
 
+// G = hr^-1 mod x^L by Newton doubling, hr of hl ≤ L words with hr[0]^-1 = g1: g_2t = g_t·(2 - hr·g_t) mod x^2t on
+// transforms of 4t points.  X and Y hold the largest of them: 2^⌈log2(2L - 1)⌉ words each.
+template <class F>
+static int newton_inverse(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u64* HR, size_t hl, size_t L, u64 g1, u64* G,
+                          u64* X, u64* Y) {
+  // g_1 (pageable source: the copy is staged before cudaMemcpyAsync returns)
+  RONK_CUDA(ctx, cudaMemcpyAsync(G, &g1, sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
+  for (size_t t = 1; t < L; t *= 2) {
+    // g_t·(2 - hr·g_t) has degree < 4t - 2: the 4t-point cyclic product is exact; keep its first m words
+    const size_t m = std::min(2 * t, L);
+    const u32 ln = log2_ceil(4 * t);
+    RONK_TRY(ntt_device_bounded(ctx, p, g, HR, std::min(hl, m), Y, (u64)1 << ln, nullptr, ln, 0));  // Ĥ of hr mod x^m
+    RONK_TRY(ntt_device_bounded(ctx, p, g, G, t, X, (u64)1 << ln, nullptr, ln, 0));                 // Ĝ of g_t
+    RONK_TRY(launch(ctx, "divrem_newton_step", divrem_newton_step_kernel<F>, grid_for(ctx, (size_t)1 << ln, 256), 256, 0, false,
+                    f, X, (const u64*)Y, (size_t)1 << ln));
+    RONK_TRY(ntt_device_bounded(ctx, p, g, X, (u64)1 << ln, G, m, nullptr, ln, 1));  // g_2t mod x^m
+  }
+  return RONK_OK;
+}
+
+int newton_inverse_device(ronk_ctx* ctx, u64 p, u64 g, const u64* hr, size_t hl, size_t L, u64 g1, u64* G, u64* X, u64* Y) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) { return newton_inverse(ctx, f, p, g, hr, hl, L, g1, G, X, Y); });
+}
+
 template <class F>
 static int divrem_newton_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db,
                                     u64 top, u64* q, u64* r) {
@@ -96,19 +120,7 @@ static int divrem_newton_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, con
   u64* HR = AR + L;
   RONK_TRY(reverse(ctx, a, da - 1, L, AR, L));
   RONK_TRY(reverse(ctx, b, db - 1, hl, HR, hl));
-  // g_1 = b[db-1]^-1 (pageable source: the copy is staged before cudaMemcpyAsync returns)
-  const u64 g1 = h_powmod(top, p - 2, p);
-  RONK_CUDA(ctx, cudaMemcpyAsync(G, &g1, sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
-  for (size_t t = 1; t < L; t *= 2) {
-    // g_t·(2 - hr·g_t) has degree < 4t - 2: the 4t-point cyclic product is exact; keep its first m words
-    const size_t m = std::min(2 * t, L);
-    const u32 ln = log2_ceil(4 * t);
-    RONK_TRY(ntt_device_bounded(ctx, p, g, HR, std::min(hl, m), Y, (u64)1 << ln, nullptr, ln, 0));  // Ĥ of hr mod x^m
-    RONK_TRY(ntt_device_bounded(ctx, p, g, G, t, X, (u64)1 << ln, nullptr, ln, 0));                 // Ĝ of g_t
-    RONK_TRY(launch(ctx, "divrem_newton_step", divrem_newton_step_kernel<F>, grid_for(ctx, (size_t)1 << ln, 256), 256, 0, false,
-                    f, X, (const u64*)Y, (size_t)1 << ln));
-    RONK_TRY(ntt_device_bounded(ctx, p, g, X, (u64)1 << ln, G, m, nullptr, ln, 1));  // g_2t mod x^m
-  }
+  RONK_TRY(newton_inverse(ctx, f, p, g, HR, hl, L, h_powmod(top, p - 2, p), G, X, Y));  // g_1 = b[db-1]^-1
   // rev(q) = ar·inv mod x^L (nq ≥ 2L - 1: no wrap into the low L words), into AR, then reversed into q
   RONK_TRY(ntt_device_bounded(ctx, p, g, AR, L, X, nq, nullptr, lq, 0));
   RONK_TRY(ntt_device_bounded(ctx, p, g, G, L, Y, nq, X, lq, 0));

@@ -78,6 +78,8 @@ struct ronk_tune {
   int msm_coord = 1;        // RONK_MSM_COORD: kzg::commit in group coordinates (two dot products mod 102 + one lookup); 0 = the paths below
   int msm_hist = 1;         // RONK_MSM_HIST: kzg::commit through the point-indexed histogram (1) or the bucket kernels (0)
   int tw_table = 0;         // RONK_TW_TABLE: inter-pass twiddles from an n-word table (1) or stepped w ← w·ρ (0)
+  int tree_min = -1;        // RONK_TREE_MIN: smallest size that takes the subproduct-tree path of from_roots / multieval /
+                            // interpolate where its transforms fit; -1 = the measured crossovers (poly.cu)
 };
 
 struct ronk_ctx {
@@ -97,6 +99,8 @@ struct ronk_ctx {
   size_t ws2_bytes = 0;
   void* ws3 = nullptr;  // third scratch buffer (polynomial division by Newton iteration, which calls the transforms)
   size_t ws3_bytes = 0;
+  void* ws4 = nullptr;  // fourth scratch buffer (subproduct tree: multipoint evaluation and interpolation, poly_tree.cu)
+  size_t ws4_bytes = 0;
   void* stage = nullptr;  // the _host entry points' arguments (stage_in); apart from ws / ws2 / ws3, so they run any path
   size_t stage_bytes = 0;
   // two-slot host pipeline (ronk_ntt_u64_host_submit / _wait)
@@ -333,5 +337,15 @@ int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len,
 bool divrem_newton_fits(u64 p, u64 g, size_t da, size_t db);  // poly_div.cu
 int divrem_newton_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64 top, u64* q,
                          u64* r);
+// G = hr^-1 mod x^L (hr: hl ≤ L words, g1 = hr[0]^-1); X, Y: 2^⌈log2(2L - 1)⌉ words each.  Stream-ordered.
+int newton_inverse_device(ronk_ctx* ctx, u64 p, u64 g, const u64* hr, size_t hl, size_t L, u64 g1, u64* G, u64* X, u64* Y);
+// Subproduct tree (poly_tree.cu) over k ≤ kTreeMaxLeaves points.  tree_fits: g != 0 and every transform of the plan
+// (tree levels above the shared-memory kernels; with d > 0 the root's division of d words) a power of two dividing
+// p - 1 and ≤ 2^26.  Arguments are checked by the caller.  from_roots with k ≤ kTreeLeaves launches no transform.
+constexpr size_t kTreeLeaves = 64, kTreeMaxLeaves = (size_t)1 << 24;
+bool tree_fits(u64 p, u64 g, size_t k, size_t d);
+int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out);
+int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u64* xs, size_t m, u64* out);
+int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u64* out);
 
 }  // namespace ronk

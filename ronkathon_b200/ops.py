@@ -69,6 +69,34 @@ def poly_eval(ctx: Context, coeffs, xs, p: int = GOLDILOCKS):
     return out
 
 
+def poly_from_roots(ctx: Context, xs, p: int = GOLDILOCKS, g: int = 7):
+    """Π (X - xs[i]) — returns a new tensor of len(xs) + 1 coefficients (subproduct tree above the crossover)."""
+    import torch
+    _check_u64(xs)
+    out = torch.empty(xs.numel() + 1, dtype=torch.int64, device=xs.device)
+    ctx.call("ronk_poly_from_roots_u64", p, g, _lib._ptr(xs), xs.numel(), _lib._ptr(out))
+    return out
+
+
+def poly_multieval(ctx: Context, coeffs, xs, p: int = GOLDILOCKS, g: int = 7):
+    """evaluate at every xs[i] — the same words as poly_eval, on a subproduct tree above the crossover."""
+    import torch
+    _check_u64(coeffs); _check_u64(xs)
+    out = torch.empty_like(xs)
+    ctx.call("ronk_poly_multieval_u64", p, g, _lib._ptr(coeffs), coeffs.numel(), _lib._ptr(xs), xs.numel(), _lib._ptr(out))
+    return out
+
+
+def poly_interpolate(ctx: Context, xs, ys, p: int = GOLDILOCKS, g: int = 7):
+    """The interpolant through (xs[i], ys[i]) — len(xs) coefficients.  Synchronous; raises RonkPanic for a repeated x."""
+    import torch
+    _check_u64(xs); _check_u64(ys)
+    assert xs.numel() == ys.numel()
+    out = torch.empty_like(xs)
+    ctx.call("ronk_poly_interpolate_u64", p, g, _lib._ptr(xs), _lib._ptr(ys), xs.numel(), _lib._ptr(out))
+    return out
+
+
 def field_binop(ctx: Context, op: str, a, b, p: int = GOLDILOCKS):
     import torch
     _check_u64(a); _check_u64(b)
