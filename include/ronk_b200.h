@@ -15,9 +15,9 @@
  *    cross-checks run through).  p = 2 is not supported (RONK_EUNSUPPORTED).
  *  - Pointers without a `_host` suffix in the function name are DEVICE pointers on the context's
  *    device; work is enqueued on the context's stream and is asynchronous unless stated.
- *    `_host` variants take host pointers, copy in, run, copy out and synchronise.  Each context keeps one
- *    staging buffer for `_host` calls, grown as needed, until ronk_ctx_destroy, like its workspace; a `_host`
- *    output buffer is written only when the call returns RONK_OK.
+ *    `_host` variants take host pointers, copy in, run, copy out and synchronise.  Each context keeps the
+ *    device scratch of its calls, the `_host` staging included, grown as needed, until ronk_ctx_destroy; a
+ *    `_host` output buffer is written only when the call returns RONK_OK.
  *  - Every function returns 0 (RONK_OK) or an error code; nothing throws, aborts or falls back
  *    to a CPU path.  Where the reference would panic/assert, RONK_EINVAL is returned.
  *  - Curve points (AffinePoint<PlutoExtendedCurve>, src/curve/mod.rs:67-74) are 4 bytes

@@ -110,11 +110,8 @@ int ronk_ctx_destroy(ronk_ctx* ctx) {
   }
   if (ctx->copy_in) cudaStreamDestroy(ctx->copy_in);
   if (ctx->copy_out) cudaStreamDestroy(ctx->copy_out);
-  if (ctx->ws) cudaFree(ctx->ws);
-  if (ctx->ws2) cudaFree(ctx->ws2);
-  if (ctx->ws3) cudaFree(ctx->ws3);
-  if (ctx->ws4) cudaFree(ctx->ws4);
-  if (ctx->stage) cudaFree(ctx->stage);
+  for (auto& b : ctx->scratch.blocks) cudaFreeAsync(b.base, ctx->stream);
+  cudaStreamSynchronize(ctx->stream);
   if (ctx->msm_ytab) cudaFree(ctx->msm_ytab);
   if (ctx->msm_done) cudaFree(ctx->msm_done);
   if (ctx->msm_coord) cudaFree(ctx->msm_coord);

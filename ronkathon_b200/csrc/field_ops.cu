@@ -268,12 +268,14 @@ int ronk_ntt_strided_small_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* 
   u64 h_wt[16];
   for (u64 j = 0; j < G; j++) h_wt[j] = h_powmod(w, j, p);
   const u64 sc = inverse ? h_powmod(G % p, p - 2, p) : 1 % p;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 16 * sizeof(u64)));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->ws2, h_wt, G * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
+  Frame fr(ctx);
+  u64* d_wt = nullptr;
+  RONK_TRY(fr.take(&d_wt, 16));
+  RONK_CUDA(ctx, cudaMemcpyAsync(d_wt, h_wt, G * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_wt is a stack buffer
   return with_field(ctx, p, 0, false, [&](const auto& f) {  // the transform's roots come from the wt table, not the policy
     return launch(ctx, "ntt_cross_rank", strided_dft_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, count, 128), 128, 0,
-                  false, f, (u64*)data, (u32)G, stride, count, (const u64*)ctx->ws2, sc);
+                  false, f, (u64*)data, (u32)G, stride, count, (const u64*)d_wt, sc);
   });
 }
 
@@ -292,9 +294,10 @@ int ronk_ntt_cross_rank_fused_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const u
   const size_t m = (size_t)1 << (log_n - log_g), blk = m >> log_g;
   const u64 wn = h_powmod(g, (p - 1) >> log_n, p);
   const u64 wg = h_powmod(g, (p - 1) >> log_g, p);
-  // ws2: [ wt: 16 words | twbase: blk words ]
-  RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, (16 + blk) * sizeof(u64)));
-  u64* d_wt = (u64*)ctx->ws2;
+  // [ wt: 16 words | twbase: blk words ]
+  Frame fr(ctx);
+  u64* d_wt = nullptr;
+  RONK_TRY(fr.take(&d_wt, 16 + blk));
   u64* d_tw = d_wt + 16;
   u64 h_wt[16];
   for (u32 j = 0; j < 16; j++) h_wt[j] = j < G ? h_powmod(wg, j, p) : 0;
@@ -327,7 +330,8 @@ int ronk_field_binop_u64_host(ronk_ctx* ctx, int op, uint64_t p, const uint64_t*
   if (!ctx || (n && (!a || !b || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
   Staged s[] = {{n * 8, a}, {n * 8, b}, {n * 8, nullptr, out}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   u64 *da = s[0].dev, *db = s[1].dev, *dout = s[2].dev;
   int rc;
   switch (op) {
@@ -345,7 +349,8 @@ int ronk_field_unop_u64_host(ronk_ctx* ctx, int op, uint64_t p, const uint64_t* 
   if (!ctx || (n && (!a || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
   Staged s[] = {{n * 8, a}, {n * 8, nullptr, out}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   const int rc = (op == 0)   ? ronk_field_neg_u64(ctx, p, s[0].dev, s[1].dev, n)
                  : (op == 1) ? ronk_field_inv_u64(ctx, p, s[0].dev, s[1].dev, n)
                              : set_err(ctx, RONK_EINVAL, "unknown op");
@@ -357,7 +362,8 @@ int ronk_field_pow_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, uint64
   if (!ctx || (n && (!a || !out))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n == 0) return RONK_OK;
   Staged s[] = {{n * 8, a}, {n * 8, nullptr, out}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   return stage_out(ctx, ronk_field_pow_u64(ctx, p, s[0].dev, e, s[1].dev, n), s);
 }
 

@@ -508,9 +508,9 @@ static int msm_hist_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points
   const size_t ctas = grid_for(ctx, n_scalars, MSM_HIST_THREADS * 8, 1);
   constexpr u32 fin_ctas = (MSM_BINS + MSM_FIN_THREADS - 1) / MSM_FIN_THREADS;  // 80
   static_assert(fin_ctas <= MSM_FIN_THREADS, "final tree assumes one CTA sum per thread");
-  const size_t need = (ctas * MSM_BINS + fin_ctas) * sizeof(u32);
-  RONK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, need));
-  u32* partial = (u32*)ctx->ws;
+  Frame fr(ctx);
+  u32* partial = nullptr;
+  RONK_TRY(fr.take(&partial, ctas * MSM_BINS + fin_ctas));
   u32* cta_sum = partial + ctas * MSM_BINS;
   // the split between shared-memory and L2 atomics pays once the SM's atomic unit is the limiter
   u32* ghist = (n_scalars >= ((size_t)1 << 22) && ctx->tune.msm_split) ? (u32*)ctx->msm_done + 1 : nullptr;
@@ -539,9 +539,9 @@ static int msm_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, con
   const int ctas = grid_for(ctx, n_scalars, MSM_THREADS * MSM_TERMS);
   // device block [flag | 17 buckets | result]: one memset, and one copy into pinned host memory at the end
   // (two copies into pageable memory cost a large share of a small call)
-  const size_t need = ((size_t)ctas * 17 + 1 + 17 + 1) * sizeof(u32);
-  RONK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, need));
-  u32* partial = (u32*)ctx->ws;
+  Frame fr(ctx);
+  u32* partial = nullptr;
+  RONK_TRY(fr.take(&partial, (size_t)ctas * 17 + 1 + 17 + 1));
   u32* d_mflag = partial + (size_t)ctas * 17;
   u32* d_buckets = d_mflag + 1;
   u32* d_result = d_buckets + 17;
@@ -602,7 +602,8 @@ int ronk_msm_pluto_ext_host(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   if (!ctx || !out || (n_scalars && (!points || !scalars))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n_points < n_scalars) return set_err(ctx, RONK_EINVAL, "srs shorter than coefficients (kzg/setup.rs:53)");
   Staged s[] = {{n_scalars * 4, points}, {n_scalars, scalars}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   return stage_out(
       ctx, ronk_msm_pluto_ext(ctx, (const uint8_t*)s[0].dev, n_scalars, (const uint8_t*)s[1].dev, n_scalars, out), s);
 }
@@ -613,7 +614,8 @@ int ronk_msm_combine_buckets_host(ronk_ctx* ctx, const uint8_t* buckets, size_t 
   if (n_sets > (1u << 20)) return set_err(ctx, RONK_EUNSUPPORTED, "too many bucket sets");
   u32 res;
   Staged s[] = {{n_sets * 17 * 4, buckets}, {17 * 4}, {4, nullptr, &res}};  // bucket sets, combined buckets, result
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   RONK_TRY(stage_out(ctx, launch(ctx, "msm_finish", msm_finish_kernel, 1, 16 * MSM_FIN_LANES, 0, false, (const u32*)s[0].dev,
                                  (u32)n_sets, (u32*)s[1].dev, (u32*)s[2].dev), s));
   unpack_to_bytes(res, out);
@@ -627,7 +629,8 @@ static int point_op_host(ronk_ctx* ctx, int op, const uint8_t* a, const uint8_t*
   if (n == 0) return RONK_OK;
   // a, b (add only), the scalars (smul only), out
   Staged s[] = {{n * 4, a}, {op == 0 ? n * 4 : 0, b}, {op == 2 ? n : 0, sc}, {n * 4, nullptr, out}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   RONK_TRY(reset_flag(ctx));
   RONK_TRY(launch(ctx, "point_op", point_op_kernel, grid_for(ctx, n, 128), 128, 0, false, op, (const u32*)s[0].dev,
                   (const u32*)s[1].dev, (const uint8_t*)s[2].dev, (u32*)s[3].dev, n, ctx->d_flag));

@@ -321,7 +321,9 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
     batch <<= LI;
   }
   if (batch > (0x7FFFFFFFu >> 12)) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
-  RONK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, ((size_t)batch << LOGN) * sizeof(u64)));
+  Frame fr(ctx);
+  u64* ws = nullptr;
+  RONK_TRY(fr.take(&ws, (size_t)batch << LOGN));
   if (LOGN >= 20 && (pl.log_n1 != (u32)(LOGN + 1) / 2 || !pl.tw_lo || !pl.tw2)) return set_err(ctx, RONK_ECUDA, "internal: unexpected plan shape");
   Ntt3Args A = {};
   A.t1 = LOGN <= ctx->tune.ntt3_t1 ? pl.t1[d] : nullptr;
@@ -334,16 +336,16 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
   A.dst_len = dst_len;
   A.mul_mask = mul_mask;
   A.src = src;
-  A.dst = (u64*)ctx->ws;
+  A.dst = ws;
   if constexpr (LOGN == 20) {
     // sixteen interleaved 2^16-point transforms + one radix-16 pass (ntt3_kernel.cuh): A1 src → data (identical views, so
     // src == data is fine), A2 data → workspace, C workspace → data.  A.tw_hi = ω_n^(1024 y): the plan's 10 / 10 split.
     A.dst = data;
     RONK_TRY((launch3<F, 2, INV, 20, false>(ctx, f, A, INV ? "intt3_a1" : "ntt3_a1", false)));
     A.src = data;
-    A.dst = (u64*)ctx->ws;
+    A.dst = ws;
     RONK_TRY((launch3<F, 1, INV, 20, false>(ctx, f, A, INV ? "intt3_a2" : "ntt3_a2", true)));
-    A.src = (const u64*)ctx->ws;
+    A.src = ws;
     A.dst = data;
     A.mul_src = mul;
     A.flags = mul ? NTT_FLAG_MUL : 0;
@@ -351,10 +353,10 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
   } else {
     if constexpr (LOGN >= 21) {
       RONK_TRY((launch3<F, 1, INV, LOGN, BOUNDED>(ctx, f, A, INV ? "intt3_pass1" : "ntt3_pass1", false)));
-      A.src = (const u64*)ctx->ws;
+      A.src = ws;
     }
     RONK_TRY((launch3<F, 2, INV, LOGN, BOUNDED && LOGN == 16>(ctx, f, A, INV ? "intt3_pass2" : "ntt3_pass2", LOGN >= 21)));
-    A.src = (const u64*)ctx->ws;
+    A.src = ws;
     A.dst = data;
     A.mul_src = mul;
     A.flags = mul ? NTT_FLAG_MUL : 0;
@@ -439,8 +441,9 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
         return run_ntt3<F, INV, 16, false>(ctx, f, pl, data, src, mul, batch, src_len, dst_len, mul_mask);
     }
   }
-  const size_t bytes = ((size_t)batch << log_n) * sizeof(u64);
-  RONK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, bytes));
+  Frame fr(ctx);
+  u64* ws = nullptr;
+  RONK_TRY(fr.take(&ws, (size_t)batch << log_n));
   // preferred tile sizes (log2): 14 / 13 (strided pass-1 reads want 32-byte segments)
   const int pref1 = ctx->tune.tile1, pref2 = ctx->tune.tile2, adapt = ctx->tune.tile_adapt;
   // The preferred sizes are tuned for grids of ≥ 1000 tiles.  A mid-size job (one 2^20 transform is 64 tiles of
@@ -456,7 +459,7 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
   u32 tile1, tile2;
   ntt_pass_tiles(log_n, p1, p2, &tile1, &tile2);
   // pass 1: N1-point transforms down the columns, inter-pass twiddle, blocked write to the workspace
-  NttTileArgs A1 = ntt_args_pass1(src, (u64*)ctx->ws, pl.tw1_2d[INV ? 1 : 0], pl.tw_lo, INV ? pl.tw_hi_inv : pl.tw2, pl.tw2,
+  NttTileArgs A1 = ntt_args_pass1(src, ws, pl.tw1_2d[INV ? 1 : 0], pl.tw_lo, INV ? pl.tw_hi_inv : pl.tw2, pl.tw2,
                                   log_n, batch, tile1, tile2, &tiles);
   A1.src_len = src_len;
   if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
@@ -467,7 +470,7 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
   }
   RONK_TRY((launch_tile<F, MODE_PASS1, INV>(ctx, f, A1, (u32)tiles, INV ? "intt_pass1" : "ntt_pass1")));
   // pass 2: N2-point transforms along the contiguous workspace tiles, natural-order output
-  NttTileArgs A2 = ntt_args_pass2((const u64*)ctx->ws, data, mul, pl.tw2_2d[INV ? 1 : 0], log_n, batch, tile2, &tiles);
+  NttTileArgs A2 = ntt_args_pass2(ws, data, mul, pl.tw2_2d[INV ? 1 : 0], log_n, batch, tile2, &tiles);
   A2.dst_len = dst_len;
   A2.mul_mask = mul_mask;
   if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");

@@ -262,8 +262,9 @@ template <class F>
 static int div_linear_with_field(ronk_ctx* ctx, const F& f, const u64* a, size_t d, u64 z, u64 scale, u64* q, u64* rem) {
   const size_t nchunks = (d + DL_CHUNK - 1) / DL_CHUNK;
   if (nchunks > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "polynomial too long");
-  RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 2 * nchunks * sizeof(u64)));
-  u64* S = (u64*)ctx->ws2;
+  Frame fr(ctx);
+  u64* S = nullptr;
+  RONK_TRY(fr.take(&S, 2 * nchunks));
   u64* carry = S + nchunks;
   RONK_TRY(launch(ctx, "div_linear_fold", div_linear_kernel<F, false>, (u32)nchunks, DL_THR, 0, false, f, a, d, z, nullptr, S,
                   scale, nullptr, nullptr));
@@ -411,8 +412,9 @@ static int poly_mul_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u6
     return launch(ctx, "poly_mul_schoolbook", poly_mul_schoolbook_kernel<F>, grid_for(ctx, L, 128), 128, 0, false, f, a, da, b,
                   db, c);
   const size_t n = (size_t)1 << log_n;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws2, &ctx->ws2_bytes, 2 * n * sizeof(u64)));
-  u64* A = (u64*)ctx->ws2;
+  Frame fr(ctx);
+  u64* A = nullptr;
+  RONK_TRY(fr.take(&A, 2 * n));
   u64* B = A + n;
   // the zero padding of a and b and the clipping of the product to L coefficients happen inside the
   // transforms' load / store phases (no pad-copy kernels, no final device copy)
@@ -519,8 +521,9 @@ static int from_roots_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t 
     return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 roots off the tree path (k sequential linear products)");
   // k linear products in one CTA (interp_master_kernel), ping-ponging between out and k + 1 words of scratch so that
   // the last one lands in out
-  RONK_TRY(ensure_ws(ctx, &ctx->ws4, &ctx->ws4_bytes, (k + 1) * sizeof(u64)));
-  u64* tmp = (u64*)ctx->ws4;
+  Frame fr(ctx);
+  u64* tmp = nullptr;
+  RONK_TRY(fr.take(&tmp, k + 1));
   return with_field(ctx, p, 0, false, [&](const auto& f) {
     return launch(ctx, "interp_master", interp_master_kernel<std::decay_t<decltype(f)>>, 1, 1024, 0, false, f, xs, (u32)k,
                   (k & 1) ? tmp : out, (k & 1) ? out : tmp);
@@ -546,8 +549,9 @@ static int interpolate_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const 
     return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 nodes off the tree path (O(K²) interpolation)");
   // the literal kernels into scratch, so that a repeated x leaves out unwritten
   const size_t nwarps = (k + 255) / 256 * 8;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws4, &ctx->ws4_bytes, (3 * k + 2 + nwarps * k) * sizeof(u64)));
-  u64* res = (u64*)ctx->ws4;
+  Frame fr(ctx);
+  u64* res = nullptr;
+  RONK_TRY(fr.take(&res, 3 * k + 2 + nwarps * k));
   u64* m0 = res + k;
   u64* m1 = m0 + k + 1;
   RONK_TRY(interp_literal(ctx, p, xs, ys, k, res, m0, m1, m1 + k + 1));
@@ -562,9 +566,11 @@ static int dft_device(ronk_ctx* ctx, u64 p, u64 g, const u64* in, u64 n, u64* ou
   if (g == 0 || g >= p) return set_err(ctx, RONK_EINVAL, "generator out of range");
   if (n == 0 || (p - 1) % n != 0)
     return set_err(ctx, RONK_EINVAL, "n must divide p - 1 (no primitive n-th root of unity)");
-  RONK_TRY(ensure_ws(ctx, &ctx->ws, &ctx->ws_bytes, n * sizeof(u64)));
-  RONK_TRY(roots_table(ctx, p, g, n, (u64*)ctx->ws));
-  return poly_eval_device(ctx, p, in, n, (const u64*)ctx->ws, n, out);  // X[i] = a(ω^i)
+  Frame fr(ctx);
+  u64* nodes = nullptr;
+  RONK_TRY(fr.take(&nodes, n));
+  RONK_TRY(roots_table(ctx, p, g, n, nodes));
+  return poly_eval_device(ctx, p, in, n, nodes, n, out);  // X[i] = a(ω^i)
 }
 
 }  // namespace ronk
@@ -622,7 +628,8 @@ int ronk_poly_mul_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t
   if (!ctx || !a || !b || !c) return set_err(ctx, RONK_EINVAL, "null argument");
   if (da == 0 || db == 0) return set_err(ctx, RONK_EINVAL, "empty polynomial (D + D2 - 1 underflows)");
   Staged s[] = {{da * 8, a}, {db * 8, b}, {(da + db - 1) * 8, nullptr, c}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   return stage_out(ctx, poly_mul_device(ctx, p, g, s[0].dev, da, s[1].dev, db, s[2].dev), s);
 }
 
@@ -631,7 +638,8 @@ int ronk_poly_eval_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* coeffs, s
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || (m && (!xs || !out)) || (d && !coeffs)) return set_err(ctx, RONK_EINVAL, "null argument");
   Staged s[] = {{d * 8, coeffs}, {m * 8, xs}, {m * 8, nullptr, out}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   return stage_out(ctx, poly_eval_device(ctx, p, s[0].dev, d, s[1].dev, m, s[2].dev), s);
 }
 
@@ -639,7 +647,8 @@ int ronk_dft_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* in,
   ronk::DeviceGuard _dg(ctx);
   if (!ctx || !in || !out) return set_err(ctx, RONK_EINVAL, "null argument");
   Staged s[] = {{n * 8, in}, {n * 8, nullptr, out}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   return stage_out(ctx, dft_device(ctx, p, g, s[0].dev, n, s[1].dev), s);
 }
 
@@ -653,7 +662,8 @@ int ronk_poly_lagrange_eval_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, cons
     return set_err(ctx, RONK_EINVAL, "n must divide p - 1 (Lagrange::new asserts)");  // mod.rs:361
   if (n > (1u << 20)) return set_err(ctx, RONK_EUNSUPPORTED, "n too large for the O(n²) barycentric form");
   Staged s[] = {{n * 8, coeffs}, {n * 8}, {8, nullptr, out}};  // coefficients, nodes, result
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   RONK_TRY(roots_table(ctx, p, g, n, s[1].dev));
   RONK_TRY(reset_flag(ctx));
   RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
@@ -679,7 +689,8 @@ int ronk_poly_interpolate_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* xs
   const size_t nwarps = (k + 255) / 256 * 8;
   // xs, ys, out, then the scratch: the master polynomial's two ping-pong buffers and the per-warp partial sums
   Staged s[] = {{k * 8, xs}, {k * 8, ys}, {k * 8, nullptr, out}, {(k + 1) * 8}, {(k + 1) * 8}, {nwarps * k * 8}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   RONK_TRY(interp_literal(ctx, p, s[0].dev, s[1].dev, k, s[2].dev, s[3].dev, s[4].dev, s[5].dev));
   return stage_out(ctx, RONK_OK, s);
 }
@@ -711,7 +722,8 @@ int ronk_poly_divrem_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* a, size
   if (da > 0x7FFFFFF0ULL || db > 0x7FFFFFF0ULL) return set_err(ctx, RONK_EUNSUPPORTED, "polynomial too long");
   if (da == 0) return RONK_OK;
   Staged s[] = {{da * 8, a}, {db * 8, b}, {da * 8, nullptr, q}, {da * 8, nullptr, r}};
-  RONK_TRY(stage_in(ctx, s));
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
   return stage_out(ctx, divrem_device(ctx, p, /*g=*/0, s[0].dev, da, s[1].dev, db, s[2].dev, s[3].dev), s);
 }
 

@@ -111,9 +111,10 @@ static int divrem_newton_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, con
   u32 lq, lr;
   divrem_newton_sizes(da, db, &lq, &lr);
   const size_t nq = (size_t)1 << lq, nr = (size_t)1 << lr, nx = std::max(nq, nr);
-  // own scratch (the transforms use ctx->ws, poly_mul ctx->ws2): X, Y transform buffers | G = inv | AR | HR
-  RONK_TRY(ensure_ws(ctx, &ctx->ws3, &ctx->ws3_bytes, (2 * nx + 2 * L + hl) * sizeof(u64)));
-  u64* X = (u64*)ctx->ws3;
+  // X, Y transform buffers | G = inv | AR | HR
+  Frame fr(ctx);
+  u64* X = nullptr;
+  RONK_TRY(fr.take(&X, 2 * nx + 2 * L + hl));
   u64* Y = X + nx;
   u64* G = Y + nx;
   u64* AR = G + L;

@@ -170,7 +170,8 @@ tree_eval_leaves_kernel(const F f, const u64* __restrict__ M, const u64* __restr
   }
 }
 
-// Shape of the tree over k leaves and its place in ctx->ws4: the stored levels lb … K, then four N-word buffers.
+// Shape of the tree over k leaves and its place in the scratch of the function that builds it: the stored levels
+// lb … K, then four N-word buffers.
 struct Tree {
   size_t k = 0, N = 1;
   u32 K = 0, lb = 0;
@@ -181,7 +182,7 @@ struct Tree {
   u64* extra = nullptr; // 3k words (interpolation)
 };
 
-static int tree_alloc(ronk_ctx* ctx, size_t k, size_t extra_words, Tree* t) {
+static int tree_alloc(Frame& fr, size_t k, size_t extra_words, Tree* t) {
   t->k = k;
   t->K = log2_ceil(k);
   t->N = (size_t)1 << t->K;
@@ -192,8 +193,7 @@ static int tree_alloc(ronk_ctx* ctx, size_t k, size_t extra_words, Tree* t) {
     at += (t->N >> j) * (((size_t)1 << j) + 1);
   }
   t->mwords = at;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws4, &ctx->ws4_bytes, (at + 4 * t->N + extra_words) * sizeof(u64)));
-  t->M = (u64*)ctx->ws4;
+  RONK_TRY(fr.take(&t->M, at + 4 * t->N + extra_words));
   for (int i = 0; i < 4; i++) t->T[i] = t->M + at + i * t->N;
   t->extra = t->M + at + 4 * t->N;
   return RONK_OK;
@@ -227,7 +227,7 @@ static int tree_build(ronk_ctx* ctx, const F& f, u64 p, u64 g, const Tree& t, co
   return RONK_OK;
 }
 
-// out[i] = f(xs[i]) down the built tree; d ≥ 1.  Uses T[0 … 3] and ctx->ws3.
+// out[i] = f(xs[i]) down the built tree; d ≥ 1.  Uses T[0 … 3].
 template <class F>
 static int tree_down(ronk_ctx* ctx, const F& f, u64 p, u64 g, const Tree& t, const u64* c, size_t d, const u64* xs, u64* out) {
   const size_t k = t.k, hl = std::min(k + 1, d);
@@ -235,8 +235,9 @@ static int tree_down(ronk_ctx* ctx, const F& f, u64 p, u64 g, const Tree& t, con
   // root: h = rev_d(f)·rev_k(M)^-1 mod y^d, ρ[u] = h[d-1-u]
   const u32 lq = std::max<u32>(1, log2_ceil(2 * d - 1));
   const size_t nq = (size_t)1 << lq;
-  RONK_TRY(ensure_ws(ctx, &ctx->ws3, &ctx->ws3_bytes, (2 * nq + 2 * d + hl) * sizeof(u64)));
-  u64* X = (u64*)ctx->ws3;
+  Frame fr(ctx);
+  u64* X = nullptr;
+  RONK_TRY(fr.take(&X, 2 * nq + 2 * d + hl));
   u64* Y = X + nq;
   u64* G = Y + nq;
   u64* FR = G + d;
@@ -274,16 +275,18 @@ bool tree_fits(u64 p, u64 g, size_t k, size_t d) {
 }
 
 int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out) {
+  Frame fr(ctx);
   Tree t;
-  RONK_TRY(tree_alloc(ctx, k, 0, &t));
+  RONK_TRY(tree_alloc(fr, k, 0, &t));
   RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) { return tree_build(ctx, f, p, g, t, xs); }));
   RONK_CUDA(ctx, cudaMemcpyAsync(out, t.M + t.off[t.K], (k + 1) * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
   return RONK_OK;
 }
 
 int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
+  Frame fr(ctx);
   Tree t;
-  RONK_TRY(tree_alloc(ctx, m, 0, &t));
+  RONK_TRY(tree_alloc(fr, m, 0, &t));
   return with_field(ctx, p, 0, false, [&](const auto& f) {
     RONK_TRY(tree_build(ctx, f, p, g, t, xs));
     return tree_down(ctx, f, p, g, t, c, d, xs, out);
@@ -291,8 +294,9 @@ int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u6
 }
 
 int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u64* out) {
+  Frame fr(ctx);
   Tree t;
-  RONK_TRY(tree_alloc(ctx, k, 2 * k, &t));
+  RONK_TRY(tree_alloc(fr, k, 2 * k, &t));
   u64* Mp = t.extra;  // M', then c_i = y_i / M'(x_i)
   u64* W = Mp + k;    // M'(x_i)
   return with_field(ctx, p, 0, false, [&](const auto& f) {

@@ -44,6 +44,18 @@ struct NttPlan {
   u64* t1[2] = {nullptr, nullptr};  // optional n-word pass-1 twiddle table (log n ≤ RONK_NTT3_T1)
 };
 
+// The context's per-call device scratch (Frame below): device blocks, of which blocks[0, used) hold the live regions,
+// the last of them in its first `top` bytes.
+struct Scratch {
+  struct Block {
+    char* base;
+    size_t bytes;
+  };
+  std::vector<Block> blocks;
+  size_t used = 0;
+  size_t top = 0;
+};
+
 }  // namespace ronk
 
 // Tuning switches, read from the environment ONCE at ronk_ctx_create (never on the launch path).
@@ -93,16 +105,7 @@ struct ronk_ctx {
   bool prof = false;
   std::vector<ronk::ProfRec> prof_log;
   std::map<std::tuple<uint64_t, uint64_t, uint32_t>, ronk::NttPlan> plans;
-  void* ws = nullptr;  // workspace (two-pass intermediate, poly_mul operands, msm partials)
-  size_t ws_bytes = 0;
-  void* ws2 = nullptr;  // second scratch buffer (poly_mul)
-  size_t ws2_bytes = 0;
-  void* ws3 = nullptr;  // third scratch buffer (polynomial division by Newton iteration, which calls the transforms)
-  size_t ws3_bytes = 0;
-  void* ws4 = nullptr;  // fourth scratch buffer (subproduct tree: multipoint evaluation and interpolation, poly_tree.cu)
-  size_t ws4_bytes = 0;
-  void* stage = nullptr;  // the _host entry points' arguments (stage_in); apart from ws / ws2 / ws3, so they run any path
-  size_t stage_bytes = 0;
+  ronk::Scratch scratch;  // every per-call device buffer: transform workspaces, operands, staged _host arguments
   // two-slot host pipeline (ronk_ntt_u64_host_submit / _wait)
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   static constexpr int kSlots = 3;
@@ -241,22 +244,83 @@ inline int grid_for(const ronk_ctx* ctx, size_t n, size_t threads, size_t per_sm
   return (int)blocks;
 }
 
-inline int ensure_ws(ronk_ctx* ctx, void** buf, size_t* cap, size_t bytes) {
-  if (*cap >= bytes) return RONK_OK;
-  if (*buf) {
-    cudaStreamSynchronize(ctx->stream);
-    cudaFree(*buf);
-    *buf = nullptr;
-    *cap = 0;
+// A scope's share of the context's scratch stack: `Frame f(ctx); u64* X; RONK_TRY(f.take(&X, words));`.  Each take
+// hands out a region above everything taken so far; the destructor gives back all the frame took.  A function takes
+// what it needs and never has to know what its callees take.  The rules:
+//  1. LIFO, no movement: a region is never moved or freed while its frame is alive, and never escapes its scope.
+//  2. Every region starts on a 256-byte boundary, as a CUDA allocation does (msm_coord_kernel's vector path needs
+//     16-byte aligned points), and spans at least 256 bytes, so that an empty request is still a valid pointer.
+//  3. A request that does not fit the rest of the current block goes to the next block.  Where there is none, it
+//     allocates one of its size.  Where the next block is too small, it frees that block and every one above it (no
+//     live frame has a region there) and allocates one of its size.  Blocks come and go in stream order
+//     (cudaMallocAsync / cudaFreeAsync on ctx->stream, from the device's default memory pool), so growing never makes
+//     the host wait: cudaFree would wait for the device, and a small block left by one call (div_linear's chunk
+//     sums) is outgrown by the next (dft's roots table) on a context fresh enough that its caller expects no wait.
+//     The pool is shared by the process: a growth may reuse memory another stream freed and so order ctx->stream
+//     behind that stream's work, as the device-wide wait of cudaFree did.
+//  4. Blocks only grow, so a call whose requests fit the blocks held does no allocation, no free and no synchronise;
+//     the blocks are freed in ronk_ctx_destroy.
+//  5. A failed allocation is RONK_ENOMEM with ctx->err set (RONK_ECUDA where the device has no memory pools); CUDA's
+//     sticky error is cleared.  The blocks a growth frees stay reserved until the stream reaches the free, so a
+//     growth that runs out of memory synchronises ctx->stream, returns the pool's unused memory and tries once more:
+//     near capacity it needs no more than the new block, as a synchronous free-then-allocate did.
+//  6. A region given back may be handed to the very next kernel on ctx->stream while an earlier kernel that used it
+//     is still queued: stream order makes that safe.  It holds because only the second and later kernels of one
+//     transform or one commit are launched with programmatic dependent launch; a kernel that starts before its
+//     predecessor ends must never be the first user of a region another call or scope gave back.
+//  7. Nothing survives a call: every function writes its scratch before it reads it.
+class Frame {
+ public:
+  ronk_ctx* const ctx;
+  explicit Frame(ronk_ctx* c) : ctx(c), used_(c->scratch.used), top_(c->scratch.top) {}
+  ~Frame() {
+    ctx->scratch.used = used_;
+    ctx->scratch.top = top_;
   }
-  cudaError_t e = cudaMalloc(buf, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return set_err(ctx, RONK_ENOMEM, "workspace allocation failed");
+  Frame(const Frame&) = delete;
+  Frame& operator=(const Frame&) = delete;
+
+  static constexpr size_t kAlign = 256;
+  static size_t span(size_t bytes) { return bytes ? (bytes + kAlign - 1) / kAlign * kAlign : kAlign; }
+
+  // *out = a region of `count` elements of T
+  template <class T>
+  int take(T** out, size_t count) {
+    Scratch& s = ctx->scratch;
+    const size_t bytes = span(count * sizeof(T));
+    if (s.used == 0 || s.blocks[s.used - 1].bytes - s.top < bytes) {
+      if (s.used < s.blocks.size() && s.blocks[s.used].bytes < bytes) {
+        for (size_t i = s.used; i < s.blocks.size(); i++) cudaFreeAsync(s.blocks[i].base, ctx->stream);
+        s.blocks.resize(s.used);
+      }
+      if (s.used == s.blocks.size()) {
+        void* p = nullptr;
+        cudaError_t e = cudaMallocAsync(&p, bytes, ctx->stream);
+        if (e == cudaErrorMemoryAllocation) {
+          cudaGetLastError();
+          cudaMemPool_t pool;
+          cudaStreamSynchronize(ctx->stream);
+          if (cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);
+          e = cudaMallocAsync(&p, bytes, ctx->stream);
+        }
+        if (e != cudaSuccess) {
+          cudaGetLastError();
+          return set_err(ctx, e == cudaErrorMemoryAllocation ? RONK_ENOMEM : RONK_ECUDA,
+                         std::string("workspace allocation failed: ") + cudaGetErrorString(e));
+        }
+        s.blocks.push_back({(char*)p, bytes});
+      }
+      s.used++;
+      s.top = 0;
+    }
+    *out = (T*)(s.blocks[s.used - 1].base + s.top);
+    s.top += bytes;
+    return RONK_OK;
   }
-  *cap = bytes;
-  return RONK_OK;
-}
+
+ private:
+  const size_t used_, top_;
+};
 
 // The device error flag that kernels raise with atomicExch: cleared before a launch, read back (synchronising the
 // stream) after it.
@@ -271,8 +335,8 @@ inline int read_flag(ronk_ctx* ctx, int* v) {
   return RONK_OK;
 }
 
-// One region of a _host call's arguments in ctx->stage: `bytes` uploaded from `in` before the call when `in` is set,
-// downloaded to `out` after a successful call when `out` is set, scratch when neither is.
+// One region of a _host call's arguments: `bytes` uploaded from `in` before the call when `in` is set, downloaded to
+// `out` after a successful call when `out` is set, scratch when neither is.
 struct Staged {
   size_t bytes;
   const void* in = nullptr;
@@ -280,23 +344,18 @@ struct Staged {
   u64* dev = nullptr;  // set by stage_in
 };
 
-// Every region starts on a 256-byte boundary, as a cudaMalloc'd buffer would (msm_coord_kernel's vector path needs
-// 16-byte aligned points), and takes at least one block, so that an empty region is still a valid pointer.
-constexpr size_t kStageAlign = 256;
-inline size_t stage_span(size_t bytes) { return (bytes / kStageAlign + 1) * kStageAlign; }
-
-// Carves the regions from ctx->stage, growing it once for all of them before any is handed out (growing frees the
-// old buffer), and enqueues the uploads on ctx->stream.
+// Carves the regions from one take of the _host entry point's frame, the outermost of the call, so that the scratch
+// grows at most once for all of them, and enqueues the uploads on ctx->stream.  The frame must outlive stage_out.
 template <size_t N>
-inline int stage_in(ronk_ctx* ctx, Staged (&r)[N]) {
+inline int stage_in(Frame& f, Staged (&r)[N]) {
   size_t total = 0;
-  for (const Staged& s : r) total += stage_span(s.bytes);
-  RONK_TRY(ensure_ws(ctx, &ctx->stage, &ctx->stage_bytes, total));
-  char* at = (char*)ctx->stage;
+  for (const Staged& s : r) total += Frame::span(s.bytes);
+  char* at = nullptr;
+  RONK_TRY(f.take(&at, total));
   for (Staged& s : r) {
     s.dev = (u64*)at;
-    at += stage_span(s.bytes);
-    if (s.in && s.bytes) RONK_CUDA(ctx, cudaMemcpyAsync(s.dev, s.in, s.bytes, cudaMemcpyHostToDevice, ctx->stream));
+    at += Frame::span(s.bytes);
+    if (s.in && s.bytes) RONK_CUDA(f.ctx, cudaMemcpyAsync(s.dev, s.in, s.bytes, cudaMemcpyHostToDevice, f.ctx->stream));
   }
   return RONK_OK;
 }

@@ -472,8 +472,8 @@ def test_repeated_x_at_size_panics(p, g, dflt):
 
 # ---- G. workspaces left dirty by larger calls -----------------------------------------------------------------------
 def test_dirty_workspaces(contexts):
-    """Small calls after a 2^24-point multieval and a 2^22-point interpolation (junk in ws, ws3 and ws4) give the words
-    the same calls give on contexts that have run nothing before them."""
+    """Small calls after a 2^24-point multieval and a 2^22-point interpolation (junk in every scratch block) give the
+    words the same calls give on contexts that have run nothing before them."""
     from ronkathon_b200 import ops
     r100, r4097 = _points(GL, 100, 180), _points(GL, 4097, 181)
     f3000, x1000 = dev(oracle.splitmix(GL, 182, 3000)), _points(GL, 1000, 183)
