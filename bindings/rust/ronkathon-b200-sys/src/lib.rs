@@ -62,6 +62,8 @@ extern "C" {
   pub fn ronk_memcpy_d2d(ctx: *mut ronk_ctx, dst: *mut c_void, src: *const c_void, bytes: usize) -> c_int;
   pub fn ronk_dft_u64(ctx: *mut ronk_ctx, p: u64, g: u64, input: *const u64, n: u64, out: *mut u64) -> c_int;
   pub fn ronk_dft_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, input: *const u64, n: u64, out: *mut u64) -> c_int;
+  pub fn ronk_ntt_any_u64(ctx: *mut ronk_ctx, p: u64, g: u64, data: *mut u64, n: u64, batch: u32, inverse: c_int) -> c_int;
+  pub fn ronk_ntt_any_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, host_data: *mut u64, n: u64, batch: u32, inverse: c_int) -> c_int;
 
   // Polynomial arithmetic (src/polynomial/arithmetic.rs, mod.rs:133-225, :382-415)
   pub fn ronk_poly_mul_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, c: *mut u64) -> c_int;

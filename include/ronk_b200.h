@@ -114,6 +114,22 @@ int ronk_ntt_mul_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *data, cons
 /* Polynomial::dft — src/polynomial/mod.rs:240-258.  Any n | p-1 (O(n²)); out must not alias in. */
 int ronk_dft_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *in, uint64_t n, uint64_t *out);
 int ronk_dft_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *in, uint64_t n, uint64_t *out);
+/* Polynomial::dft (src/polynomial/mod.rs:240-258) and its inverse for ANY n | p - 1, in place, `batch` contiguous
+ * transforms of n points, natural order: X[k] = Σ_j a_j ω^(jk), ω = g^((p-1)/n); inverse uses ω^-1 and scales by n^-1.
+ * g generates F_p*, as for ronk_poly_mul_u64.  The forward result is, for every n, the words ronk_dft_u64 gives for
+ * each transform (any g whose g^((p-1)/N) has order N will do, N below); for n a power of two both directions are the
+ * words of ronk_ntt_u64.  Path, in O(n log n) except the third:
+ *   - n a power of two: ronk_ntt_u64's transform (n ≤ 2^26);
+ *   - Bluestein, when N = 2^⌈log2(2n - 1)⌉ ≤ 2^26 divides p - 1 and n reaches a measured crossover (DESIGN.md §5):
+ *     two batched N-point transforms and two memory-bound chirp passes.  For Goldilocks that is every n | p - 1 up to
+ *     2^25.  Scratch: batch·N words.  The spectrum of the chirp, N words (512 MiB at n = 3·2^23), is kept on the context
+ *     per (p, g, n) until ronk_ctx_destroy;
+ *   - otherwise ronk_dft_u64's O(n²) kernels, up to n ≤ 2^17.
+ * RONK_EINVAL: a null pointer, n == 0, n not dividing p - 1, g == 0 or g >= p.  RONK_EUNSUPPORTED: p = 2, or n off all
+ * three paths.  batch == 0 does nothing.  Nothing is written on failure.  The device variant is asynchronous on the
+ * context's stream; the _host variant stages in and out and synchronises. */
+int ronk_ntt_any_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *data, uint64_t n, uint32_t batch, int inverse);
+int ronk_ntt_any_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *host_data, uint64_t n, uint32_t batch, int inverse);
 
 /* Distributed-transform building blocks (SURVEY §8e: the top log2(G) stages of one large NTT across
  * G GPUs).  out[i] = scale * base^i — the twiddle column ω_n^(r·k') a rank multiplies into its

@@ -57,6 +57,8 @@ SIGNATURES = {
     "ronk_memcpy_d2d": (i32, [vp, vp, vp, sz]),
     "ronk_dft_u64": (i32, [vp, u64, u64, vp, u64, vp]),
     "ronk_dft_u64_host": (i32, [vp, u64, u64, vp, u64, vp]),
+    "ronk_ntt_any_u64": (i32, [vp, u64, u64, vp, u64, u32, i32]),
+    "ronk_ntt_any_u64_host": (i32, [vp, u64, u64, vp, u64, u32, i32]),
     "ronk_poly_mul_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_mul_u64_host": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_add_u64": (i32, [vp, u64, vp, sz, vp, sz, vp]),

@@ -62,6 +62,7 @@ int ronk_ctx_create(ronk_ctx** out, int device, void* stream) {
   ctx->tune.msm_hist = env_int("RONK_MSM_HIST", 1);
   ctx->tune.msm_split = env_int("RONK_MSM_SPLIT", 0);
   ctx->tune.tree_min = env_int("RONK_TREE_MIN", -1);
+  ctx->tune.anyntt_min = env_int("RONK_ANYNTT_MIN", -1);
   ctx->stream = (cudaStream_t)stream;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return RONK_ECUDA; }
@@ -101,6 +102,7 @@ int ronk_ctx_destroy(ronk_ctx* ctx) {
       if (p.t1[d]) cudaFree(p.t1[d]);
     }
   }
+  for (auto& kv : ctx->anyntt_spec) cudaFree(kv.second);
   for (auto& r : ctx->prof_log) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
   for (int i = 0; i < ronk_ctx::kSlots; i++) {
     if (ctx->slot_buf[i]) cudaFree(ctx->slot_buf[i]);

@@ -441,7 +441,7 @@ static int poly_addsub(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64*
   });
 }
 
-static int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
+int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
   if (!ctx || (m && (!xs || !out)) || (d && !c)) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(validate_modulus(ctx, p));
   if (m == 0) return RONK_OK;
@@ -452,7 +452,7 @@ static int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const 
 }
 
 // nodes[i] = ω_n^i (plain residues)
-static int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes) {
+int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes) {
   u64 w;
   if (ronk_root_of_unity(p, g, n, (uint64_t*)&w) != RONK_OK)
     return set_err(ctx, RONK_EINVAL, "n must divide p - 1 (no primitive n-th root of unity)");

@@ -92,6 +92,8 @@ struct ronk_tune {
   int tw_table = 0;         // RONK_TW_TABLE: inter-pass twiddles from an n-word table (1) or stepped w ← w·ρ (0)
   int tree_min = -1;        // RONK_TREE_MIN: smallest size that takes the subproduct-tree path of from_roots / multieval /
                             // interpolate where its transforms fit; -1 = the measured crossovers (poly.cu)
+  int anyntt_min = -1;      // RONK_ANYNTT_MIN: smallest n that takes Bluestein in ronk_ntt_any_u64 where its convolution fits;
+                            // -1 = the measured crossover (ntt_any.cu)
 };
 
 struct ronk_ctx {
@@ -105,6 +107,7 @@ struct ronk_ctx {
   bool prof = false;
   std::vector<ronk::ProfRec> prof_log;
   std::map<std::tuple<uint64_t, uint64_t, uint32_t>, ronk::NttPlan> plans;
+  std::map<std::tuple<uint64_t, uint64_t, uint64_t>, uint64_t*> anyntt_spec;  // (p, g, n) → Bluestein spectrum, N words (ntt_any.cu)
   ronk::Scratch scratch;  // every per-call device buffer: transform workspaces, operands, staged _host arguments
   // two-slot host pipeline (ronk_ntt_u64_host_submit / _wait)
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
@@ -393,6 +396,9 @@ int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n
 int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst, const u64* mul, u32 log_n, u32 batch);
 int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len, u64* dst, u64 dst_len, const u64* mul,
                        u32 log_n, int inverse);
+// poly.cu: nodes[i] = ω_n^i (plain residues), n ≤ 2^31 - 1; out[i] = Σ_j c_j xs[i]^j, one CTA per point
+int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes);
+int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs, size_t m, u64* out);
 bool divrem_newton_fits(u64 p, u64 g, size_t da, size_t db);  // poly_div.cu
 int divrem_newton_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64 top, u64* q,
                          u64* r);

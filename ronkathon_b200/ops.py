@@ -34,6 +34,15 @@ def ntt_(ctx: Context, data, log_n: int, batch: int = 1, inverse: bool = False, 
     return data
 
 
+def ntt_any_(ctx: Context, data, n: int, batch: int = 1, inverse: bool = False, p: int = GOLDILOCKS, g: int = 7):
+    """In-place transforms of any length n | p - 1 (Polynomial::dft and its inverse) over `batch` contiguous rows:
+    the power-of-two transform, Bluestein's algorithm where its convolution fits, else the O(n²) dft kernels."""
+    _check_u64(data)
+    assert data.numel() == batch * n
+    ctx.call("ronk_ntt_any_u64", p, g, _lib._ptr(data), n, batch, int(inverse))
+    return data
+
+
 def ntt_mul_(ctx: Context, data, mul, log_n: int, batch: int = 1, p: int = GOLDILOCKS, g: int = 7):
     """data ← NTT(data) ⊙ mul, the point-wise product fused into the last stage."""
     _check_u64(data); _check_u64(mul)

@@ -106,6 +106,15 @@ class Polynomial:
                          _lib._ptr(out))
         return self._like(out, Lagrange)
 
+    def idft(self):
+        """Lagrange → Monomial for any n | p-1: the inverse of `dft`, a_j = n^-1 Σ_k X_k ω^(-jk).  An extension: the
+        reference has no inverse for n that is not a power of two.  O(n log n) wherever ronk_ntt_any_u64 runs
+        Bluestein's algorithm."""
+        assert self.basis is Lagrange
+        data = self.coefficients.copy()
+        self._ctx().call("ronk_ntt_any_u64_host", self.p, self.g, _lib._ptr(data), len(data), 1, 1)
+        return self._like(data, Monomial)
+
     def _ntt(self, inverse: bool):
         n = len(self.coefficients)
         if n == 0 or n & (n - 1):  # where [(); D.is_power_of_two() as usize - 1]: (mod.rs:274)
