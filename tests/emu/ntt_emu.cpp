@@ -338,6 +338,28 @@ int run16_cluster(const F& f, u64 p, u64 g, u64* data, const u64* mul, u32 batch
   return 0;
 }
 
+template <int S>
+void gl_pow2_n(const u64* a, u64* out, u64 n) {
+  GoldilocksField f;
+  for (u64 i = 0; i < n; i++) out[i] = f.mul_pow2<S>(a[i]);
+}
+template <int E, bool INV>
+void gl_w16_sub_n(const u64* a, const u64* b, u64* out, u64 n) {
+  GoldilocksField f;
+  for (u64 i = 0; i < n; i++) out[i] = f.w16_sub<E, INV>(a[i], b[i]);
+}
+template <int... S>
+void gl_pow2_dispatch(int s, const u64* a, u64* out, u64 n, std::integer_sequence<int, S...>) {
+  static void (*const table[])(const u64*, u64*, u64) = {&gl_pow2_n<S>...};
+  table[s](a, out, n);
+}
+template <int... E>
+void gl_w16_sub_dispatch(int e, bool inv, const u64* a, const u64* b, u64* out, u64 n, std::integer_sequence<int, E...>) {
+  static void (*const fwd[])(const u64*, const u64*, u64*, u64) = {&gl_w16_sub_n<E, false>...};
+  static void (*const bwd[])(const u64*, const u64*, u64*, u64) = {&gl_w16_sub_n<E, true>...};
+  (inv ? bwd : fwd)[e](a, b, out, n);
+}
+
 }  // namespace
 
 
@@ -540,6 +562,21 @@ void emu_gl_w16(uint64_t a, uint64_t out[16]) {
   out[4] = f.w16<4, false>(a); out[5] = f.w16<5, false>(a); out[6] = f.w16<6, false>(a); out[7] = f.w16<7, false>(a);
   out[8] = f.w16<0, true>(a); out[9] = f.w16<1, true>(a); out[10] = f.w16<2, true>(a); out[11] = f.w16<3, true>(a);
   out[12] = f.w16<4, true>(a); out[13] = f.w16<5, true>(a); out[14] = f.w16<6, true>(a); out[15] = f.w16<7, true>(a);
+}
+
+// The host twins of the Goldilocks shift primitives, element-wise, on the inputs the device harness gets
+// (tests/cuda/field_harness.cu).  op 0: out = mul_pow2<k>(a), k in [0, 192); op 1: out = w16_sub<k, inv>(a, b),
+// k in [0, 8).
+int emu_gl_shift_op(int op, int k, int inv, const uint64_t* a, const uint64_t* b, uint64_t* out, uint64_t n) {
+  if (op == 0 && k >= 0 && k < 192) {
+    gl_pow2_dispatch(k, a, out, n, std::make_integer_sequence<int, 192>{});
+    return 0;
+  }
+  if (op == 1 && k >= 0 && k < 8) {
+    gl_w16_sub_dispatch(k, inv != 0, a, b, out, n, std::make_integer_sequence<int, 8>{});
+    return 0;
+  }
+  return 1;
 }
 
 // Bank-conflict audit of the shared-memory swizzle: worst number of distinct 8-byte banks hit

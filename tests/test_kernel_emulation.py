@@ -3,44 +3,21 @@ field.cuh / ntt_kernel.cuh for the host and runs the tile phases thread by threa
 maps, round schedule, twiddle tables and field arithmetic against the oracle.  The emulator is
 test infrastructure; the product library never executes on the CPU."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import field_corpus as fc
 import oracle
 from gpu_util import BABYBEAR, PBIG
 
-HERE =os.path.dirname(os.path.abspath(__file__))
 GL = oracle.GOLDILOCKS
 P64 = C.POINTER(C.c_uint64)
 
 
 @pytest.fixture(scope="module")
 def emu():
-    src = os.path.join(HERE, "emu", "ntt_emu.cpp")
-    so = os.path.join(HERE, "emu", "libntt_emu.so")
-    hdr = os.path.join(HERE, "..", "ronkathon_b200", "csrc", "ntt_kernel.cuh")
-    hdr2 = os.path.join(HERE, "..", "ronkathon_b200", "csrc", "field.cuh")
-    hdr3 = os.path.join(HERE, "..", "ronkathon_b200", "csrc", "ntt12_kernel.cuh")
-    hdr4 = os.path.join(HERE, "..", "ronkathon_b200", "csrc", "ntt3_kernel.cuh")
-    newest = max(os.path.getmtime(x) for x in (src, hdr, hdr2, hdr3, hdr4))
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so, src])
-    lib = C.CDLL(so)
-    lib.emu_ntt.argtypes = [C.c_uint64, C.c_uint64, P64, P64, C.c_uint32, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32]
-    lib.emu_ntt_bounded.argtypes = [C.c_uint64, C.c_uint64, P64, C.c_uint64, P64, C.c_uint64, P64, C.c_uint32, C.c_int,
-                                    C.c_uint32, C.c_uint32, C.c_uint32]
-    lib.emu_field_op.argtypes = [C.c_uint64, C.c_int, P64, P64, P64, C.c_uint64, C.c_int]
-    lib.emu_gl_w16.argtypes = [C.c_uint64, P64]
-    lib.emu_swizzle_worst_conflict.argtypes = [C.c_uint32, C.c_uint32]
-    lib.emu_fast12_tiles.restype = C.c_uint64
-    lib.emu_ntt3.argtypes = [P64, P64, C.c_uint32, C.c_uint32, C.c_int, C.c_int]
-    lib.emu_ntt3_bounded.argtypes = [P64, C.c_uint64, P64, C.c_uint64, P64, C.c_int]
-    lib.emu_ntt16_cluster.argtypes = [P64, P64, C.c_uint32, C.c_int]
-    lib.emu_ntt3_shared_mul.argtypes = [P64, P64, C.c_uint32, C.c_uint32]
-    return lib
+    return fc.host_twin()
 
 
 def _ptr(a):
@@ -55,21 +32,20 @@ def emu_ntt(emu, p, g, data, log_n, batch=1, inverse=False, mul=None, tile_cap=1
     return d
 
 
-def edge_values(p):
-    vals = [0, 1, 2, p - 1, p - 2, p // 2, p // 2 + 1]
-    if p > (1 << 33):
-        vals += [(1 << 32) - 1, 1 << 32, (1 << 32) + 1, p - (1 << 32), p - (1 << 32) + 1, p - (1 << 32) - 1,
-                 (1 << 63), (1 << 63) + 1, 0xFFFFFFFF00000000, 0xFFFFFFFE00000002, 0x00000000FFFFFFFF]
-    return [v % p for v in vals]
+_EXTRA_MONT = [p for p in fc.MONT_PRIMES.values() if p not in (GL, 101, 17, 127, 0xFFFFFFFFFFFFFFC5, 0x7FFFFFFFFFFFFFE7,
+                                                                4179340454199820289)]
 
 
 @pytest.mark.parametrize("p,force_mont", [(GL, 0), (GL, 1), (101, 0), (17, 0), (127, 0),
-                                          (0xFFFFFFFFFFFFFFC5, 0), (0x7FFFFFFFFFFFFFE7, 0), (4179340454199820289, 0)])
+                                          (0xFFFFFFFFFFFFFFC5, 0), (0x7FFFFFFFFFFFFFE7, 0), (4179340454199820289, 0)]
+                         + [(p, 0) for p in _EXTRA_MONT])
 def test_field_policies_match_oracle(emu, p, force_mont):
+    """The host twin of both field policies on the structured corpus of tests/field_corpus.py (every pair of its
+    values) plus random odd words, against the oracle."""
     rng = np.random.default_rng(5)
-    ev = edge_values(p)
-    a = [x for x in ev for _ in ev] + [int(v) % p for v in rng.integers(0, 2**63, 4000, dtype=np.uint64) * 2 + 1]
-    b = [y for _ in ev for y in ev] + [int(v) % p for v in rng.integers(0, 2**63, 4000, dtype=np.uint64) * 2 + 1]
+    sa, sb = fc.gl_pairs() if p == GL else fc.mont_pairs(p)
+    a = [int(x) for x in sa] + [int(v) % p for v in rng.integers(0, 2**63, 4000, dtype=np.uint64) * 2 + 1]
+    b = [int(y) for y in sb] + [int(v) % p for v in rng.integers(0, 2**63, 4000, dtype=np.uint64) * 2 + 1]
     a, b = np.array(a, dtype=np.uint64), np.array(b, dtype=np.uint64)
     out = np.empty_like(a)
     for op, fn in ((0, oracle.add), (1, oracle.sub), (2, oracle.mul)):
@@ -84,11 +60,66 @@ def test_goldilocks_shift_twiddles(emu):
     w16 = oracle.root_of_unity(GL, 16)
     w16i = oracle.inverse(GL, w16)
     out = np.empty(16, dtype=np.uint64)
-    for a in edge_values(GL) + [int(v) for v in oracle.splitmix(GL, 9, 50)]:
+    for a in list(fc.gl_values()) + [int(v) for v in oracle.splitmix(GL, 9, 50)]:
         emu.emu_gl_w16(a, _ptr(out))
         for e in range(8):
             assert int(out[e]) == oracle.mul(GL, a, oracle.pow_(GL, w16, e)), (a, e)
             assert int(out[8 + e]) == oracle.mul(GL, a, oracle.pow_(GL, w16i, e)), (a, e)
+
+
+@pytest.mark.parametrize("S", range(192))
+def test_goldilocks_host_mul_pow2_on_the_shift_corpus(S):
+    """The host twin of mul_pow2<S> on the inputs the device harness gets for S, against Python integers."""
+    x = np.array(fc.gl_shift_inputs(S), dtype=np.uint64)
+    assert np.array_equal(fc.host_gl_shift(0, S, False, x), fc.exact("mul", GL, x, [pow(2, S, GL)] * len(x))), S
+
+
+@pytest.mark.parametrize("inverse", [False, True])
+@pytest.mark.parametrize("e", range(8))
+def test_goldilocks_host_w16_sub_on_the_shift_corpus(e, inverse):
+    """w16_sub<E, INV>(a, b) = (a − b)·ω16^±E, with a − b (or b − a, where the sign is folded into the subtraction)
+    running over the shift corpus of its S."""
+    a, b = fc.gl_w16_sub_operands(fc.w16_shift(e, inverse))
+    w = pow(oracle.root_of_unity(GL, 16), -e if inverse else e, GL)
+    assert np.array_equal(fc.host_gl_shift(1, e, inverse, a, b), fc.exact("mul", GL, fc.exact("sub", GL, a, b),
+                                                                            [w] * len(a)))
+
+
+def test_corpus_reaches_every_case():
+    """Every case the derivations in field.cuh name is reached at least MIN_HITS times by the corpus handed to its
+    op; a case fewer inputs below p reach is listed with its size in field_corpus and must be reached exactly that
+    often (the corpus holds all of it).  The test primes are prime."""
+    def check(counts, expected, small, what):
+        for case in expected:
+            need, _ = small.get(case, (None, None))
+            got = counts.get(case, 0)
+            if need is None:
+                assert got >= fc.MIN_HITS, (what, case, got)
+            else:
+                assert got == need, (what, case, got, need)
+    a, b = fc.gl_pairs()
+    check(fc.count_cases(fc.gl_add_cases, a, b), ("sum_lt_p", "sum_in_p_2_64", "sum_carries_2_64"), {}, "gl add")
+    check(fc.count_cases(fc.sub_cases, a, b), ("a_ge_b", "a_lt_b"), {}, "gl sub")
+    check(fc.count_cases(fc.gl_mul_cases, a, b), fc.GL_MUL_CASES, fc.GL_MUL_SMALL, "gl mul")
+    for S in range(192):
+        counts = fc.count_cases(lambda x: fc.gl_shift_cases(S, x), fc.gl_shift_inputs(S))
+        small = {c: v for (s, c), v in fc.GL_SHIFT_SMALL.items() if s == S}
+        check(counts, fc.SHIFT_CASES[fc.gl_shift_form(S)], small, f"mul_pow2<{S}>")
+    for e in range(8):   # w16_sub hands mul_pow2 the difference: the same inputs, reached through the subtraction
+        for inverse in (False, True):
+            S = fc.w16_shift(e, inverse)
+            a, b = fc.gl_w16_sub_operands(S)
+            d = fc.exact("sub", GL, b, a) if S >= 96 else fc.exact("sub", GL, a, b)
+            assert set(int(v) for v in d) >= set(fc.gl_shift_inputs(S)), (e, inverse)
+    for name, p in fc.MONT_PRIMES.items():
+        assert fc.is_prime(p), name
+        a, b = fc.mont_pairs(p)
+        if p < fc.EXHAUSTIVE_BELOW:      # every pair of residues: each case holds all the inputs it can
+            assert len(a) == p * p
+            continue
+        check(fc.count_cases(lambda x, y: fc.mont_add_cases(p, x, y), a, b), fc.mont_add_expected_cases(p), {}, name)
+        check(fc.count_cases(fc.sub_cases, a, b), ("a_ge_b", "a_lt_b"), {}, name)
+        check(fc.count_cases(lambda x, y: fc.redc_cases(p, x, y), a, b), fc.mont_redc_expected_cases(p), {}, name)
 
 
 def test_swizzle_is_conflict_free(emu):
