@@ -87,6 +87,12 @@ extern "C" {
   /// Division by b0 + b1·x (the divisor `kzg::open` builds, src/kzg/setup.rs:72-75) as a device-wide scan; device pointers.
   pub fn ronk_poly_div_linear_u64(ctx: *mut ronk_ctx, p: u64, a: *const u64, d: usize, b0: u64, b1: u64, q: *mut u64, rem: *mut u64) -> c_int;
 
+  // Reed–Solomon codes (src/codes/reed_solomon.rs:42-52): encoding, and errors-and-erasures decoding up to
+  // n - k ≤ RONK_RS_MAX_PARITY; status[b] = errors corrected, or -1 for a row outside the decoding radius.
+  pub fn ronk_rs_encode_u64(ctx: *mut ronk_ctx, p: u64, g: u64, msg: *const u64, k: u64, n: u64, batch: u32, codeword: *mut u64) -> c_int;
+  pub fn ronk_rs_decode_u64(ctx: *mut ronk_ctx, p: u64, g: u64, received: *const u64, erased: *const u8, n: u64, k: u64, batch: u32, msg: *mut u64, status: *mut i32) -> c_int;
+  pub fn ronk_rs_decode_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, received: *const u64, erased: *const u8, n: u64, k: u64, batch: u32, msg: *mut u64, status: *mut i32) -> c_int;
+
   // AffinePoint<PlutoExtendedCurve> + kzg::commit (src/curve/mod.rs:157-235, src/kzg/setup.rs:48-60)
   pub fn ronk_point_add_pluto_ext_host(ctx: *mut ronk_ctx, a: *const u8, b: *const u8, out: *mut u8, n: usize) -> c_int;
   pub fn ronk_point_neg_pluto_ext_host(ctx: *mut ronk_ctx, a: *const u8, out: *mut u8, n: usize) -> c_int;

@@ -255,6 +255,36 @@ int ronk_poly_multieval_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_
 int ronk_poly_interpolate_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *ys, size_t k, uint64_t *out);
 int ronk_poly_div_linear_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t d, uint64_t b0, uint64_t b1, uint64_t *q, uint64_t *rem);
 
+/* ---- Reed–Solomon codes ------------------------------------------------------------------- */
+/* Position i < n of a codeword holds the value at ω_n^i, ω_n = g^((p-1)/n): the domain of Message::encode
+ * (src/codes/reed_solomon.rs:42-52).  Row-major, DEVICE pointers, asynchronous on the context's stream.
+ * Arguments: RONK_EINVAL for a null pointer, n == 0, k == 0, k > n, n not dividing p - 1, g == 0 or g >= p, ω_n of order
+ * below n (two positions would share a point; g must generate a subgroup of order divisible by n), or an output that
+ * overlaps an input.  RONK_EUNSUPPORTED for p = 2, n off ronk_ntt_any_u64's paths, or 3·batch·n ≥ 2^31 (decode;
+ * batch·n for encode).  batch == 0 does nothing.  Every check is made before anything is enqueued; nothing is written
+ * on failure.  The transforms are ronk_ntt_any_u64's: below its crossover, for n not a power of two, a batched O(n²)
+ * kernel takes every row in one launch, so the launch sequence of a call does not depend on the batch (save where
+ * ronk_ntt_u64 itself picks its kernels by batch, at 2^16 points). */
+/* Message::encode of `batch` messages msg (batch × k): codeword[b][i] = m_b(ω_n^i), i < n (batch × n). */
+int ronk_rs_encode_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *msg, uint64_t k, uint64_t n, uint32_t batch,
+                       uint64_t *codeword);
+/* Errors-and-erasures decoding of `batch` received words (batch × n).  erased (batch × n bytes) may be NULL, meaning no
+ * erasures; a nonzero byte marks that position as erased.  Writes msg (batch × k) and status (batch entries).
+ * Guarantee: if row b differs from the codeword of a message m in e non-erased positions, with ε erased positions and
+ * 2e + ε ≤ n - k, then msg[b] = m and status[b] = e.  Otherwise the row gets status[b] = -1 with msg[b] all zero, or a
+ * message m' with status[b] = e' whose codeword differs from the row in e' non-erased positions, 2e' + ε ≤ n - k: the
+ * decoder is bounded-distance and never returns a message outside the decoding radius.  A failed row is a result, not
+ * an error; the call never reads back to the host.
+ * n - k is at most RONK_RS_MAX_PARITY (the Berlekamp–Massey locator runs in one CTA per row, in shared memory);
+ * above it RONK_EUNSUPPORTED.  Scratch: 4·batch·n words + batch·16 bytes (below the crossover also n + 3·batch·(n-k+1)
+ * words), plus the transforms' own (Bluestein: 3·batch·N words, N = 2^⌈log2(2n - 1)⌉).
+ * The _host variant takes host pointers, stages in and out and synchronises. */
+#define RONK_RS_MAX_PARITY 8191
+int ronk_rs_decode_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *received, const uint8_t *erased, uint64_t n,
+                       uint64_t k, uint32_t batch, uint64_t *msg, int32_t *status);
+int ronk_rs_decode_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *received, const uint8_t *erased,
+                            uint64_t n, uint64_t k, uint32_t batch, uint64_t *msg, int32_t *status);
+
 /* ---- curve + kzg::commit ------------------------------------------------------------------ */
 /* AffinePoint Add / Neg / Mul<ScalarField> — src/curve/mod.rs:178-213, :225-235, :157-172,
  * element-wise over n points (host pointers).  RONK_EINVAL for off-curve / malformed input. */

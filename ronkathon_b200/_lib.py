@@ -73,6 +73,9 @@ SIGNATURES = {
     "ronk_poly_from_roots_u64": (i32, [vp, u64, u64, vp, sz, vp]),
     "ronk_poly_multieval_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_interpolate_u64": (i32, [vp, u64, u64, vp, vp, sz, vp]),
+    "ronk_rs_encode_u64": (i32, [vp, u64, u64, vp, u64, u64, u32, vp]),
+    "ronk_rs_decode_u64": (i32, [vp, u64, u64, vp, vp, u64, u64, u32, vp, vp]),
+    "ronk_rs_decode_u64_host": (i32, [vp, u64, u64, vp, vp, u64, u64, u32, vp, vp]),
     "ronk_point_add_pluto_ext_host": (i32, [vp, vp, vp, vp, sz]),
     "ronk_point_neg_pluto_ext_host": (i32, [vp, vp, vp, sz]),
     "ronk_point_smul_pluto_ext_host": (i32, [vp, vp, vp, vp, sz]),

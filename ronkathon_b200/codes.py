@@ -5,6 +5,8 @@
   message zero-padded to N coefficients (a plain NTT when N is a power of two).
 * Reed–Solomon `Message::decode` (reed_solomon.rs:55-107): Lagrange interpolation through the first
   K coordinates (`ronk_poly_interpolate_u64_host`).
+* Reed–Solomon errors-and-erasures correction (`rs_correct`): reads all N coordinates and corrects up to the
+  decoding radius (`ronk_rs_decode_u64_host`).
 * Shamir `split` (src/shamir/mod.rs:53-58): `Polynomial::evaluate` at x = 1..n, one batched kernel.
 """
 from __future__ import annotations
@@ -40,6 +42,34 @@ def rs_decode(codeword, k: int, field):
     _lib.default_context().call("ronk_poly_interpolate_u64_host", field.ORDER, _lib._ptr(xs), _lib._ptr(ys), k,
                                 _lib._ptr(out))
     return [field(int(v)) for v in out]
+
+
+def rs_correct(codeword, k: int, field, erasures=()):
+    """Errors-and-erasures decoding of one received word [(x_i, y_i)] whose x_i are ω_n^i in order (as rs_encode
+    gives them): returns (message, errors), the message as k field elements and the number of errors corrected, or
+    (None, -1) when no codeword lies within the decoding radius (2·errors + len(erasures) ≤ n - k).  `erasures` are
+    positions whose y is unknown.  Beyond rs_decode, which trusts the first k coordinates, this reads all n and corrects
+    them: one batched device decode (ronk_rs_decode_u64_host)."""
+    from . import _lib
+    n = len(codeword)
+    assert 0 < k <= n, "need 0 < k <= n"
+    p, g = field.ORDER, field.PRIMITIVE_ELEMENT.value
+    xs = np.array([int(getattr(x, "value", x)) for x, _ in codeword], dtype=np.uint64)
+    ys = np.array([int(getattr(y, "value", y)) for _, y in codeword], dtype=np.uint64)
+    ctx = _lib.default_context()
+    dom = np.zeros(n, dtype=np.uint64)           # ω_n^i: the transform of the monomial X (of 1 when n = 1)
+    dom[1 % n] = 1
+    ctx.call("ronk_ntt_any_u64_host", p, g, _lib._ptr(dom), n, 1, 0)
+    assert np.array_equal(xs, dom), "x coordinates must be ω_n^i, i = 0 … n-1, in order"
+    erased = np.zeros(n, dtype=np.uint8)
+    erased[list(erasures)] = 1
+    msg = np.empty(k, dtype=np.uint64)
+    status = np.empty(1, dtype=np.int32)
+    ctx.call("ronk_rs_decode_u64_host", p, g, _lib._ptr(ys), _lib._ptr(erased), n, k, 1, _lib._ptr(msg),
+             _lib._ptr(status))
+    if status[0] < 0:
+        return None, -1
+    return [field(int(v)) for v in msg], int(status[0])
 
 
 def shamir_shares(coefficients, n: int, field):

@@ -116,10 +116,9 @@ static u32 log2_ceil_u64(u64 v) {
   return k;
 }
 
-// Which kernels run a transform of n points (anyntt_path): the power-of-two transform; Bluestein when its convolution of
-// N = 2^⌈log2(2n - 1)⌉ ≤ 2^26 points divides p - 1 and n reaches the crossover; the literal evaluation at n roots of unity
-// (ronk_dft_u64's kernels) up to kAnyNttLiteralMax; else nothing.
-enum AnyNttPath { AN_POW2, AN_BLUESTEIN, AN_LITERAL, AN_NONE };
+// Which kernels run a transform of n points (anyntt_path, AnyNttPath in ronk_internal.h): the power-of-two transform;
+// Bluestein when its convolution of N = 2^⌈log2(2n - 1)⌉ ≤ 2^26 points divides p - 1 and n reaches the crossover; the
+// literal evaluation at n roots of unity (ronk_dft_u64's kernels) up to kAnyNttLiteralMax; else nothing.
 constexpr u64 kAnyNttLiteralMax = (u64)1 << 17;
 // Smallest n that takes Bluestein where it fits: tools/anyntt_timing.py on an H100 80GB HBM3 at 700 W (DESIGN.md §5), the
 // smallest n from which Bluestein won at every larger n measured (4080: 0.081 vs 0.081 ms; 3840: 0.082 vs 0.077).
@@ -136,7 +135,7 @@ static AnyNttPath anyntt_path(const ronk_ctx* ctx, u64 p, u64 n) {
 }
 
 // Checks of both variants; *path set on RONK_OK.
-static int anyntt_args(ronk_ctx* ctx, u64 p, u64 g, const void* data, u64 n, AnyNttPath* path) {
+int anyntt_args(ronk_ctx* ctx, u64 p, u64 g, const void* data, u64 n, AnyNttPath* path) {
   if (!ctx || !data) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(validate_modulus(ctx, p));
   if (g == 0 || g >= p) return set_err(ctx, RONK_EINVAL, "generator out of range");
@@ -227,7 +226,7 @@ static int anyntt_literal(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 bat
   });
 }
 
-static int anyntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int inverse) {
+int anyntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int inverse) {
   AnyNttPath path;
   RONK_TRY(anyntt_args(ctx, p, g, data, n, &path));
   if (batch == 0) return RONK_OK;

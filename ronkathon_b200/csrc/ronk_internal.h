@@ -412,5 +412,9 @@ bool tree_fits(u64 p, u64 g, size_t k, size_t d);
 int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out);
 int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u64* xs, size_t m, u64* out);
 int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u64* out);
+// ntt_any.cu: ronk_ntt_any_u64 on device pointers, and its argument and path check (*path set on RONK_OK).
+enum AnyNttPath { AN_POW2, AN_BLUESTEIN, AN_LITERAL, AN_NONE };
+int anyntt_args(ronk_ctx* ctx, u64 p, u64 g, const void* data, u64 n, AnyNttPath* path);
+int anyntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int inverse);
 
 }  // namespace ronk

@@ -106,6 +106,35 @@ def poly_interpolate(ctx: Context, xs, ys, p: int = GOLDILOCKS, g: int = 7):
     return out
 
 
+def rs_encode(ctx: Context, msg, n: int, batch: int = 1, p: int = GOLDILOCKS, g: int = 7):
+    """Reed–Solomon Message::encode of `batch` messages (msg: batch × k, row-major): a new batch × n tensor of
+    codewords, position i holding the message polynomial at ω_n^i."""
+    import torch
+    _check_u64(msg)
+    assert msg.numel() % batch == 0
+    out = torch.empty(batch * n, dtype=torch.int64, device=msg.device)
+    ctx.call("ronk_rs_encode_u64", p, g, _lib._ptr(msg), msg.numel() // batch if batch else 0, n, batch, _lib._ptr(out))
+    return out
+
+
+def rs_decode(ctx: Context, received, k: int, erased=None, batch: int = 1, p: int = GOLDILOCKS, g: int = 7):
+    """Errors-and-erasures decoding of `batch` received words (batch × n): returns new tensors (messages, batch × k;
+    status, int32 per row: the errors corrected, or -1 with a zero message for a row outside the decoding radius).
+    erased: None or a uint8/bool tensor of batch × n, nonzero at erased positions.  Asynchronous."""
+    import torch
+    _check_u64(received)
+    assert received.numel() % batch == 0 if batch else received.numel() == 0
+    n = received.numel() // batch if batch else 0
+    if erased is not None:
+        erased = erased.to(torch.uint8).contiguous()
+        assert erased.is_cuda and erased.numel() == received.numel()
+    msg = torch.empty(batch * k, dtype=torch.int64, device=received.device)
+    status = torch.empty(batch, dtype=torch.int32, device=received.device)
+    ctx.call("ronk_rs_decode_u64", p, g, _lib._ptr(received), _lib._ptr(erased), n, k, batch, _lib._ptr(msg),
+             _lib._ptr(status))
+    return msg, status
+
+
 def field_binop(ctx: Context, op: str, a, b, p: int = GOLDILOCKS):
     import torch
     _check_u64(a); _check_u64(b)
