@@ -194,9 +194,19 @@ int ronk_ntt_u64_dist_virtual(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *d
 int ronk_msm_pluto_ext_dist(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t out[4]);
 
 /* ---- Polynomial<Monomial, F, D> ----------------------------------------------------------- */
-/* Mul — src/polynomial/arithmetic.rs:97-119.  c has da+db-1 coefficients (no trimming).
- * NTT path (pad → NTT, NTT∘pointwise → iNTT) when a power of two ≥ da+db-1 divides p-1 and
- * the product is large enough to pay for it, else the schoolbook kernel (e.g. p = 101). */
+/* Mul — src/polynomial/arithmetic.rs:97-119.  c has L = da+db-1 coefficients (no trimming), the same words on every path.
+ * - NTT path (pad → NTT, NTT∘pointwise → iNTT over p, with g's roots of unity) when g != 0, a power of two N ≥ L
+ *   divides p-1 and the product is large enough to pay for it.
+ * - Multi-modular path when g != 0, no power of two ≥ L divides p-1 (p = 101, or an NTT prime past its 2-adicity),
+ *   L ≤ 2^26, da·db ≥ 2^16 / 2^20 / 2^20 and min(da, db) ≥ 256 / 512 / 1024 for k = 1 / 2 / 3 (the measured
+ *   crossovers; RONK_CRT_MUL_MIN replaces both with one bound on da·db): the integer product is convolved modulo the k ≤ 3 NTT primes 0xFFFFFFFF00000001,
+ *   0xFFFFFFFF70000001 and 29·2^57+1, k the fewest whose product exceeds min(da, db)·(p-1)² (k = 1 up to p ≈ 2^19.5,
+ *   k = 2 up to p ≈ 2^51.5 at min(da, db) = 2^25), and rebuilt by the Chinese remainder theorem.  Here g is only an
+ *   on/off switch: the transforms use the auxiliary primes' own generators.  Device scratch: 2·N + k·L words, plus
+ *   the transforms' own workspace of up to N words (3 GiB at L = 2^26, k = 3).
+ * - Otherwise (and always for g = 0) the schoolbook kernel.
+ * Asynchronous on every path.  On the two transform paths c may alias a or b (both operands are consumed before the
+ * last launch writes c); on the schoolbook path c must not overlap a or b. */
 int ronk_poly_mul_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *c);
 int ronk_poly_mul_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *c);
 /* Add/Sub/Neg — src/polynomial/arithmetic.rs:16-94: out has da terms, b zero-extended/truncated. */

@@ -63,6 +63,8 @@ int ronk_ctx_create(ronk_ctx** out, int device, void* stream) {
   ctx->tune.msm_split = env_int("RONK_MSM_SPLIT", 0);
   ctx->tune.tree_min = env_int("RONK_TREE_MIN", -1);
   ctx->tune.anyntt_min = env_int("RONK_ANYNTT_MIN", -1);
+  const char* crt_min = getenv("RONK_CRT_MUL_MIN");
+  ctx->tune.crt_mul_min = crt_min ? strtoll(crt_min, nullptr, 10) : -1;
   ctx->stream = (cudaStream_t)stream;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return RONK_ECUDA; }

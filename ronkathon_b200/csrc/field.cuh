@@ -428,5 +428,15 @@ inline u64 h_inv64(u64 p) {  // p^-1 mod 2^64 (p odd), Newton
   for (int i = 0; i < 6; i++) x *= 2 - p * x;
   return x;
 }
+// The Montgomery policy of an odd modulus p without roots of unity: every w16t entry is R mod p (the identity).
+inline MontField h_mont_field(u64 p) {
+  MontField f;
+  f.p = p;
+  f.pinv = h_inv64(p);
+  const u64 r1 = (u64)((((unsigned __int128)1) << 64) % p);
+  f.r2 = h_mulmod(r1, r1, p);
+  for (int e = 0; e < 8; e++) f.w16t[e] = r1;
+  return f;
+}
 
 }  // namespace ronk

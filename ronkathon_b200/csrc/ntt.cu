@@ -14,12 +14,8 @@ namespace ronk {
 
 int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out) {
   if (!(p & 1) || p < 3) return set_err(ctx, RONK_EUNSUPPORTED, "modulus must be an odd prime");
-  MontField f;
-  f.p = p;
-  f.pinv = h_inv64(p);
-  const u64 r1 = (u64)((((unsigned __int128)1) << 64) % p);
-  f.r2 = h_mulmod(r1, r1, p);
-  for (int e = 0; e < 8; e++) f.w16t[e] = r1;
+  MontField f = h_mont_field(p);
+  const u64 r1 = f.w16t[0];  // R mod p
   if (g) {
     u32 k = 0;
     while (k < 4 && ((p - 1) >> k) % 2 == 0) k++;

@@ -408,9 +408,11 @@ static int poly_mul_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u6
   // NTT cost ~ 3·n·log n / 2 multiplies vs da·db for schoolbook
   const double school = (double)da * (double)db;
   const double viantt = 1.5 * (double)((size_t)1 << log_n) * (double)log_n + 4096.0;
-  if (!ntt_ok || school <= viantt)
+  if (!ntt_ok || school <= viantt) {
+    if (crt_mul_fits(ctx, p, g, da, db)) return crt_mul_device(ctx, p, a, da, b, db, c);  // poly_crt.cu
     return launch(ctx, "poly_mul_schoolbook", poly_mul_schoolbook_kernel<F>, grid_for(ctx, L, 128), 128, 0, false, f, a, da, b,
                   db, c);
+  }
   const size_t n = (size_t)1 << log_n;
   Frame fr(ctx);
   u64* A = nullptr;

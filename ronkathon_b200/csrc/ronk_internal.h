@@ -94,6 +94,9 @@ struct ronk_tune {
                             // interpolate where its transforms fit; -1 = the measured crossovers (poly.cu)
   int anyntt_min = -1;      // RONK_ANYNTT_MIN: smallest n that takes Bluestein in ronk_ntt_any_u64 where its convolution fits;
                             // -1 = the measured crossover (ntt_any.cu)
+  long long crt_mul_min = -1;  // RONK_CRT_MUL_MIN: smallest da·db that takes the multi-modular path of ronk_poly_mul_u64 where it
+                               // fits, whatever min(da, db) (64-bit: da·db reaches 2^52); -1 = the measured crossovers on
+                               // da·db and min(da, db) (poly_crt.cu)
 };
 
 struct ronk_ctx {
@@ -416,5 +419,11 @@ int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, 
 enum AnyNttPath { AN_POW2, AN_BLUESTEIN, AN_LITERAL, AN_NONE };
 int anyntt_args(ronk_ctx* ctx, u64 p, u64 g, const void* data, u64 n, AnyNttPath* path);
 int anyntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int inverse);
+// poly_crt.cu: the multi-modular product.  crt_mul_fits: g != 0, L = da + db - 1 ≤ kCrtMulMaxLen, no power of two ≥ L
+// divides p - 1, and da·db and min(da, db) reach the crossovers.  crt_mul_device: c = a·b (L words) on device pointers, stream-ordered;
+// arguments are checked by the caller.
+constexpr size_t kCrtMulMaxLen = (size_t)1 << 26;
+bool crt_mul_fits(const ronk_ctx* ctx, u64 p, u64 g, size_t da, size_t db);
+int crt_mul_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, u64* c);
 
 }  // namespace ronk
