@@ -206,7 +206,8 @@ int ronk_msm_pluto_ext_dist(ronk_ctx *ctx, const uint8_t *points, size_t n_point
  *   the transforms' own workspace of up to N words (3 GiB at L = 2^26, k = 3).
  * - Otherwise (and always for g = 0) the schoolbook kernel.
  * Asynchronous on every path.  On the two transform paths c may alias a or b (both operands are consumed before the
- * last launch writes c); on the schoolbook path c must not overlap a or b. */
+ * last launch writes c); on the schoolbook path c must not overlap a or b.  a, b and c need only the 8-byte alignment
+ * of a uint64_t, and no word behind a[da), b[db) or c[L) is ever read or written. */
 int ronk_poly_mul_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *c);
 int ronk_poly_mul_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *c);
 /* Add/Sub/Neg — src/polynomial/arithmetic.rs:16-94: out has da terms, b zero-extended/truncated. */
