@@ -68,6 +68,8 @@ extern "C" {
   // Polynomial arithmetic (src/polynomial/arithmetic.rs, mod.rs:133-225, :382-415)
   pub fn ronk_poly_mul_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, c: *mut u64) -> c_int;
   pub fn ronk_poly_mul_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, c: *mut u64) -> c_int;
+  pub fn ronk_poly_mul_batch_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, b_shared: c_int, batch: u32, c: *mut u64) -> c_int;
+  pub fn ronk_poly_mul_batch_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, b_shared: c_int, batch: u32, c: *mut u64) -> c_int;
   pub fn ronk_poly_add_u64(ctx: *mut ronk_ctx, p: u64, a: *const u64, da: usize, b: *const u64, db: usize, out: *mut u64) -> c_int;
   pub fn ronk_poly_sub_u64(ctx: *mut ronk_ctx, p: u64, a: *const u64, da: usize, b: *const u64, db: usize, out: *mut u64) -> c_int;
   pub fn ronk_poly_eval_u64(ctx: *mut ronk_ctx, p: u64, coeffs: *const u64, d: usize, xs: *const u64, m: usize, out: *mut u64) -> c_int;

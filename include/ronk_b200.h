@@ -210,6 +210,29 @@ int ronk_msm_pluto_ext_dist(ronk_ctx *ctx, const uint8_t *points, size_t n_point
  * of a uint64_t, and no word behind a[da), b[db) or c[L) is ever read or written. */
 int ronk_poly_mul_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *c);
 int ronk_poly_mul_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *c);
+/* `batch` products at once: c[r] = a[r] · b[b_shared ? 0 : r], r < batch.  Rows are contiguous: a is batch × da,
+ * b is batch × db (or db words when b_shared), c is batch × L, L = da + db − 1, each row untrimmed.
+ * - Same words: every row holds exactly the words ronk_poly_mul_u64 gives for that row's pair, on every prime and path.
+ * - Paths, chosen once per call from (p, g, da, db); N = 2^⌈log2 L⌉:
+ *   fused: g != 0, N ≤ 2^11 divides p − 1 and da·db is above the crossover: ONE launch for the whole batch, each CTA
+ *     multiplying 2^11/N products in shared memory (no scratch);
+ *   batched transforms: g != 0, 2^11 < N ≤ 2^26 divides p − 1, above the crossover: zero-padded rows, batched forward
+ *     transforms (b's with the point-wise product fused in), batched inverse, clipped rows.  Scratch 2·batch·N words
+ *     (batch·N + N with a shared b) plus the transforms' workspace of batch·N words;
+ *   multi-modular: g != 0, no power of two ≥ L divides p − 1, L ≤ 2^26, above the crossover: the two paths above modulo
+ *     each of ronk_poly_mul_u64's k ≤ 3 auxiliary primes and one Chinese-remainder pass.  Scratch k·batch·L words,
+ *     batch·da + batch·db (or + db) more where an auxiliary prime is below p, plus what the paths above take;
+ *   otherwise (always for g = 0 and L > 2^26) the schoolbook kernel over batch·L outputs.
+ *   RONK_POLY_BATCH_PATH forces a path where it applies (INTEGRATION.md).
+ * - Errors: RONK_EINVAL for a null pointer, da == 0 or db == 0, an invalid modulus, g >= p, or a c that overlaps a or
+ *   b (unlike the single product, c may never alias an operand: its rows are longer).  RONK_EUNSUPPORTED for
+ *   da or db above 2^32, more than 2^40 words in a, b or c, or more than 2^32 words of batched transforms (batch·N on
+ *   the batched-transform and multi-modular paths with N > 2^11).
+ * - Every check is made and all scratch (RONK_ENOMEM) is taken before anything is enqueued; on failure nothing is
+ *   written.  batch == 0 does nothing.  Asynchronous (the _host variant stages its arguments and synchronises).
+ * - No word past a[batch·da), b[batch·db) (b[db) when shared) or c[batch·L) is read or written; 8-byte alignment. */
+int ronk_poly_mul_batch_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, int b_shared, uint32_t batch, uint64_t *c);
+int ronk_poly_mul_batch_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, int b_shared, uint32_t batch, uint64_t *c);
 /* Add/Sub/Neg — src/polynomial/arithmetic.rs:16-94: out has da terms, b zero-extended/truncated. */
 int ronk_poly_add_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *out);
 int ronk_poly_sub_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *out);

@@ -61,6 +61,8 @@ SIGNATURES = {
     "ronk_ntt_any_u64_host": (i32, [vp, u64, u64, vp, u64, u32, i32]),
     "ronk_poly_mul_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_mul_u64_host": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
+    "ronk_poly_mul_batch_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, i32, u32, vp]),
+    "ronk_poly_mul_batch_u64_host": (i32, [vp, u64, u64, vp, sz, vp, sz, i32, u32, vp]),
     "ronk_poly_add_u64": (i32, [vp, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_sub_u64": (i32, [vp, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_eval_u64": (i32, [vp, u64, vp, sz, vp, sz, vp]),

@@ -65,6 +65,7 @@ int ronk_ctx_create(ronk_ctx** out, int device, void* stream) {
   ctx->tune.anyntt_min = env_int("RONK_ANYNTT_MIN", -1);
   const char* crt_min = getenv("RONK_CRT_MUL_MIN");
   ctx->tune.crt_mul_min = crt_min ? strtoll(crt_min, nullptr, 10) : -1;
+  ctx->tune.poly_batch_path = env_int("RONK_POLY_BATCH_PATH", 0);
   ctx->stream = (cudaStream_t)stream;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return RONK_ECUDA; }

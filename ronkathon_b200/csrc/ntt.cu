@@ -509,6 +509,21 @@ int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst,
   });
 }
 
+// The single-tile plan of (p, g, 2^log_n), built on first use: its per-round forward and inverse twiddle tables and n^-1
+// in twiddle form.  Used by the fused batched product (poly_batch.cu).
+int ntt_single_tables(ronk_ctx* ctx, u64 p, u64 g, u32 log_n, const u64** fwd, const u64** inv, u64* scale_inv) {
+  if (log_n == 0 || ntt_shape(log_n).two_pass || (p - 1) % ((u64)1 << log_n) != 0)
+    return set_err(ctx, RONK_EINVAL, "internal: not a single-tile transform size");
+  return with_field(ctx, p, g, false, [&](const auto& f) {
+    NttPlan* pl = nullptr;
+    RONK_TRY(plan_for(ctx, f, p, g, log_n, &pl));
+    *fwd = pl->tw1_2d[0];
+    *inv = pl->tw1_2d[1];
+    *scale_inv = pl->scale_inv;
+    return RONK_OK;
+  });
+}
+
 int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n, u32 batch, int inverse) {
   if (!ctx || !data) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(validate_modulus(ctx, p));

@@ -17,16 +17,22 @@ __global__ void poly_addsub_kernel(const F f, const u64* a, size_t da, const u64
   }
 }
 
-// Schoolbook product (arithmetic.rs:110-118): one thread per output coefficient.
+// Schoolbook product (arithmetic.rs:110-118) of `total / L` contiguous rows: c[r] = a[r]·b[r] (b_stride = db) or
+// a[r]·b (b_stride = 0), one thread per output coefficient.  A single product is one row (total = L).
 template <class F>
-__global__ void poly_mul_schoolbook_kernel(const F f, const u64* a, size_t da, const u64* b, size_t db, u64* c) {
+__global__ void poly_mul_schoolbook_kernel(const F f, const u64* a, size_t da, const u64* b, size_t db, size_t b_stride,
+                                           u64* c, u64 total) {
   const size_t L = da + db - 1;
   const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < L; k += stride) {
+  for (u64 o = (size_t)blockIdx.x * blockDim.x + threadIdx.x; o < total; o += stride) {
+    const u64 r = total == L ? 0 : (total >> 32) ? o / L : (u32)o / (u32)L;
+    const size_t k = o - r * L;
+    const u64* ar = a + r * da;
+    const u64* br = b + r * b_stride;
     const size_t lo = (k >= db) ? k - db + 1 : 0, hi = (k < da) ? k : da - 1;
     u64 acc = 0;
-    for (size_t i = lo; i <= hi; i++) acc = f.add(acc, f.mul(a[i], b[k - i]));
-    c[k] = acc;
+    for (size_t i = lo; i <= hi; i++) acc = f.add(acc, f.mul(ar[i], br[k - i]));
+    c[o] = acc;
   }
 }
 
@@ -286,8 +292,6 @@ static int div_linear_device(ronk_ctx* ctx, u64 p, const u64* a, size_t d, u64 b
   return with_field(ctx, p, 0, false, [&](const auto& f) { return div_linear_with_field(ctx, f, a, d, z, b1inv, q, rem); });
 }
 
-static bool overlaps(const u64* x, size_t nx, const u64* y, size_t ny) { return nx && ny && x < y + ny && y < x + nx; }
-
 // quotient_and_remainder (mod.rs:170-225) on device pointers, q and r of da words.  The host reads b[db-1] to choose:
 // a zero top word keeps the reference's quirks (literal kernel); otherwise the division is Euclidean and goes to the
 // cheapest exact path — nothing to do for da < db, the scan for a linear divisor, Newton iteration on the transforms
@@ -411,7 +415,7 @@ static int poly_mul_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u6
   if (!ntt_ok || school <= viantt) {
     if (crt_mul_fits(ctx, p, g, da, db)) return crt_mul_device(ctx, p, a, da, b, db, c);  // poly_crt.cu
     return launch(ctx, "poly_mul_schoolbook", poly_mul_schoolbook_kernel<F>, grid_for(ctx, L, 128), 128, 0, false, f, a, da, b,
-                  db, c);
+                  db, db, c, (u64)L);
   }
   const size_t n = (size_t)1 << log_n;
   Frame fr(ctx);
@@ -423,6 +427,15 @@ static int poly_mul_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u6
   RONK_TRY(ntt_device_bounded(ctx, p, g, a, da, A, n, nullptr, log_n, 0));  // Â
   RONK_TRY(ntt_device_bounded(ctx, p, g, b, db, B, n, A, log_n, 0));        // B̂ ⊙ Â fused into the last stage
   return ntt_device_bounded(ctx, p, g, B, n, c, L, nullptr, log_n, 1);      // back to coefficients, L of them
+}
+
+int poly_mul_schoolbook_rows(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, size_t b_stride,
+                             u64 batch, u64* c) {
+  const u64 total = batch * (u64)(da + db - 1);
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "poly_mul_schoolbook", poly_mul_schoolbook_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, total, 128),
+                  128, 0, false, f, a, da, b, db, b_stride, c, total);
+  });
 }
 
 static int poly_mul_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64* c) {

@@ -101,4 +101,52 @@ int crt_mul_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, 
   });
 }
 
+// The same path over `batch` contiguous rows (ronk_poly_mul_batch_u64): one crt_reduce over the flat batch·da and
+// batch·db (db when shared) words where q_i < p, the batched product over q_i into C_i (batch·L words), one crt_combine
+// over batch·L words.
+size_t crt_mul_rows_scratch(const ronk_ctx* ctx, u64 p, size_t da, size_t db, bool b_shared, u32 batch) {
+  const size_t L = da + db - 1, nb = b_shared ? db : (size_t)batch * db;
+  const int K = crt_prime_count(p, std::min(da, db));
+  size_t w = (size_t)K * batch * L;
+  bool reduce = false;
+  for (int i = 0; i < K; i++) reduce = reduce || kCrtQ[i] < p;
+  if (reduce) w += (size_t)batch * da + nb;
+  return w + poly_mul_rows_pow2_scratch(ctx, da, db, b_shared, batch) + 3 * Frame::kAlign / 8;
+}
+
+int crt_mul_rows_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, bool b_shared, u32 batch,
+                        u64* c) {
+  const size_t L = da + db - 1, na = (size_t)batch * da, nb = b_shared ? db : (size_t)batch * db, total = (size_t)batch * L;
+  const int K = crt_prime_count(p, std::min(da, db));
+  Frame fr(ctx);
+  u64* C = nullptr;
+  RONK_TRY(fr.take(&C, (size_t)K * total));
+  u64 *ra = nullptr, *rb = nullptr;
+  for (int i = 0; i < K; i++) {
+    const u64 q = kCrtQ[i], g = kCrtG[i];
+    const u64 *sa = a, *sb = b;
+    if (q < p) {
+      if (!ra) {
+        RONK_TRY(fr.take(&ra, na));
+        RONK_TRY(fr.take(&rb, nb));
+      }
+      RONK_TRY(launch(ctx, "crt_reduce", crt_reduce_kernel, grid_for(ctx, std::max(na, nb), CRT_THREADS), CRT_THREADS, 0, false,
+                      q, a, na, ra, b, nb, rb));
+      sa = ra;
+      sb = rb;
+    }
+    RONK_TRY(poly_mul_rows_pow2(ctx, q, g, sa, da, sb, db, b_shared, batch, C + (size_t)i * total));
+  }
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    const CrtConsts k = crt_consts(f);
+    const int grid = grid_for(ctx, total, CRT_THREADS);
+    switch (K) {
+      case 1: return launch(ctx, "crt_combine", crt_combine_kernel<F, 1>, grid, CRT_THREADS, 0, false, f, k, C, total, c);
+      case 2: return launch(ctx, "crt_combine", crt_combine_kernel<F, 2>, grid, CRT_THREADS, 0, false, f, k, C, total, c);
+      default: return launch(ctx, "crt_combine", crt_combine_kernel<F, 3>, grid, CRT_THREADS, 0, false, f, k, C, total, c);
+    }
+  });
+}
+
 }  // namespace ronk

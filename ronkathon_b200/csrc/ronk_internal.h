@@ -97,6 +97,9 @@ struct ronk_tune {
   long long crt_mul_min = -1;  // RONK_CRT_MUL_MIN: smallest da·db that takes the multi-modular path of ronk_poly_mul_u64 where it
                                // fits, whatever min(da, db) (64-bit: da·db reaches 2^52); -1 = the measured crossovers on
                                // da·db and min(da, db) (poly_crt.cu)
+  int poly_batch_path = 0;  // RONK_POLY_BATCH_PATH: path of ronk_poly_mul_batch_u64 where it applies: 0 = the measured crossovers,
+                            // 1 = schoolbook, 2 = transforms (fused up to its cap, multi-modular where no root fits), 3 = the
+                            // batched transforms even where the fused kernel fits (poly_batch.cu)
 };
 
 struct ronk_ctx {
@@ -377,6 +380,9 @@ inline int stage_out(ronk_ctx* ctx, int rc, const Staged (&r)[N]) {
   return RONK_OK;
 }
 
+// Whether the nx words at x and the ny words at y share a word.
+inline bool overlaps(const u64* x, size_t nx, const u64* y, size_t ny) { return nx && ny && x < y + ny && y < x + nx; }
+
 int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out);  // ntt.cu
 int validate_modulus(ronk_ctx* ctx, u64 p);                                       // field_ops.cu
 
@@ -399,6 +405,8 @@ int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n
 int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst, const u64* mul, u32 log_n, u32 batch);
 int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len, u64* dst, u64 dst_len, const u64* mul,
                        u32 log_n, int inverse);
+// The single-tile plan of 2^log_n points (log_n ≤ 13): per-round twiddle tables (forward, inverse) and n^-1, twiddle form.
+int ntt_single_tables(ronk_ctx* ctx, u64 p, u64 g, u32 log_n, const u64** fwd, const u64** inv, u64* scale_inv);
 // poly.cu: nodes[i] = ω_n^i (plain residues), n ≤ 2^31 - 1; out[i] = Σ_j c_j xs[i]^j, one CTA per point
 int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes);
 int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs, size_t m, u64* out);
@@ -425,5 +433,19 @@ int anyntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int 
 constexpr size_t kCrtMulMaxLen = (size_t)1 << 26;
 bool crt_mul_fits(const ronk_ctx* ctx, u64 p, u64 g, size_t da, size_t db);
 int crt_mul_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, u64* c);
+// Batched products (poly_batch.cu): `batch` contiguous rows c[r] = a[r]·b[b_shared ? 0 : r], L = da + db - 1 words each.
+// poly_mul_rows_pow2: on the fused kernel or the batched transforms over q, where a power of two N ≥ L divides q - 1
+// (N ≤ 2^26, batch·N within poly_batch.cu's envelope).  crt_mul_rows_device (poly_crt.cu): the multi-modular path over
+// the same rows.  *scratch_words: the words either takes from the context's scratch, its transforms' workspace included.
+// Arguments are checked by the caller; stream-ordered; c is written by the last launch only.
+int poly_mul_rows_pow2(ronk_ctx* ctx, u64 q, u64 g, const u64* a, size_t da, const u64* b, size_t db, bool b_shared,
+                       u32 batch, u64* c);
+size_t poly_mul_rows_pow2_scratch(const ronk_ctx* ctx, size_t da, size_t db, bool b_shared, u32 batch);
+int crt_mul_rows_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, bool b_shared, u32 batch,
+                        u64* c);
+size_t crt_mul_rows_scratch(const ronk_ctx* ctx, u64 p, size_t da, size_t db, bool b_shared, u32 batch);
+// poly.cu: the schoolbook kernel over `batch` contiguous rows (b_stride = db, or 0 for one shared b).
+int poly_mul_schoolbook_rows(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, size_t b_stride,
+                             u64 batch, u64* c);
 
 }  // namespace ronk

@@ -244,7 +244,7 @@ rs_finish_kernel(const u64* __restrict__ C, u64 n, u64 k, const RsRow* __restric
   if (blockIdx.y == 0 && threadIdx.x == 0) status[b] = ok ? (int32_t)(rw.deg - rw.eps) : -1;
 }
 
-static bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
+static bool bytes_overlap(const void* a, size_t na, const void* b, size_t nb) {
   if (!a || !b || !na || !nb) return false;
   const char *x = (const char*)a, *y = (const char*)b;
   return x < y + nb && y < x + na;
@@ -284,7 +284,7 @@ static int rs_encode_device(ronk_ctx* ctx, u64 p, u64 g, const u64* msg, u64 k, 
   if (!ctx || !msg || !cw) return set_err(ctx, RONK_EINVAL, "null argument");
   AnyNttPath path;
   RONK_TRY(rs_args(ctx, p, g, msg, n, k, batch, &path));
-  if (overlaps(msg, (size_t)batch * k * 8, cw, (size_t)batch * n * 8)) return set_err(ctx, RONK_EINVAL, "output overlaps input");
+  if (bytes_overlap(msg, (size_t)batch * k * 8, cw, (size_t)batch * n * 8)) return set_err(ctx, RONK_EINVAL, "output overlaps input");
   if (batch == 0) return RONK_OK;
   if (path != AN_LITERAL) {
     RONK_TRY(launch(ctx, "rs_pad", rs_pad_kernel, grid_for(ctx, (size_t)batch * n, RS_THREADS), RS_THREADS, 0, false, msg, k,
@@ -303,8 +303,8 @@ static int rs_decode_args(ronk_ctx* ctx, u64 p, u64 g, const void* received, con
   if (!ctx || !received || !msg || !status) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(rs_args(ctx, p, g, received, n, k, 3 * (u64)batch, path));
   const size_t nr = (size_t)batch * n * 8, ne = (size_t)batch * n, nm = (size_t)batch * k * 8, ns = (size_t)batch * 4;
-  if (overlaps(msg, nm, received, nr) || overlaps(msg, nm, erased, ne) || overlaps(status, ns, received, nr) ||
-      overlaps(status, ns, erased, ne) || overlaps(msg, nm, status, ns))
+  if (bytes_overlap(msg, nm, received, nr) || bytes_overlap(msg, nm, erased, ne) || bytes_overlap(status, ns, received, nr) ||
+      bytes_overlap(status, ns, erased, ne) || bytes_overlap(msg, nm, status, ns))
     return set_err(ctx, RONK_EINVAL, "output overlaps input");
   if (n - k > kRsMaxParity) return set_err(ctx, RONK_EUNSUPPORTED, "n - k above kRsMaxParity = 8191");
   return RONK_OK;

@@ -59,6 +59,21 @@ def poly_mul(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
     return out
 
 
+def poly_mul_batch(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
+    """Polynomial::mul of every row pair: a is (batch, da); b is (batch, db), or (db,) for one b shared by every row.
+    Returns a new (batch, da + db - 1) tensor, row r = a[r]·b[r] (or a[r]·b), each row the words poly_mul gives."""
+    import torch
+    _check_u64(a); _check_u64(b)
+    assert a.dim() == 2 and b.dim() in (1, 2), "a is (batch, da); b is (batch, db) or (db,)"
+    batch, da = a.shape
+    shared = b.dim() == 1
+    db = b.shape[-1]
+    assert shared or b.shape[0] == batch
+    out = torch.empty((batch, da + db - 1), dtype=torch.int64, device=a.device)
+    ctx.call("ronk_poly_mul_batch_u64", p, g, _lib._ptr(a), da, _lib._ptr(b), db, int(shared), batch, _lib._ptr(out))
+    return out
+
+
 def poly_divrem(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
     """Polynomial::quotient_and_remainder — returns new tensors (q, r), each with len(a) coefficients (zero-padded
     like the reference's arrays).  Synchronous; raises RonkPanic where the reference panics."""
