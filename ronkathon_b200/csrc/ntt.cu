@@ -484,15 +484,22 @@ static int ntt_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, u64* data, co
 }
 
 // One transform, out of place: dst[0, dst_len) = NTT(src[0, src_len) zero-extended to 2^log_n) [⊙ mul].
-// log_n >= 1; dst needs only dst_len words.  Used by poly_mul (poly.cu).
+// log_n >= 1; dst needs only dst_len words.  Used by product_bounded and the Newton inversion (poly_div.cu).
 int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len, u64* dst, u64 dst_len, const u64* mul,
                        u32 log_n, int inverse) {
   if (!ctx || !src || !dst) return set_err(ctx, RONK_EINVAL, "null argument");
-  if (log_n == 0 || log_n > 26 || (p - 1) % ((u64)1 << log_n) != 0)
-    return set_err(ctx, RONK_EINVAL, "unsupported transform size");
+  if (log_n == 0 || !pow2_fits(p, log_n)) return set_err(ctx, RONK_EINVAL, "unsupported transform size");
   return with_field(ctx, p, g, inverse != 0, [&](const auto& f) {
     return ntt_with_field(ctx, f, p, g, dst, mul, log_n, 1, inverse, src, src_len, dst_len);
   });
+}
+
+int product_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* a, u64 la, const u64* b, u64 lb, u32 log_n, u64* X, u64* Y,
+                    u64* out, u64 out_len) {
+  const u64 n = (u64)1 << log_n;
+  RONK_TRY(ntt_device_bounded(ctx, p, g, a, la, X, n, nullptr, log_n, 0));  // Â
+  RONK_TRY(ntt_device_bounded(ctx, p, g, b, lb, Y, n, X, log_n, 0));        // B̂ ⊙ Â fused into the last pass
+  return ntt_device_bounded(ctx, p, g, Y, n, out, out_len, nullptr, log_n, 1);
 }
 
 // dst = NTT(src) ⊙ mul (forward), batch transforms, mul an n-word table shared by all of them (index & (n-1)).
@@ -500,8 +507,7 @@ int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len,
 // store phase of the local transform instead of two extra passes over the data.
 int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst, const u64* mul, u32 log_n, u32 batch) {
   if (!ctx || !src || !dst) return set_err(ctx, RONK_EINVAL, "null argument");
-  if (log_n == 0 || log_n > 26 || (p - 1) % ((u64)1 << log_n) != 0)
-    return set_err(ctx, RONK_EINVAL, "unsupported transform size");
+  if (log_n == 0 || !pow2_fits(p, log_n)) return set_err(ctx, RONK_EINVAL, "unsupported transform size");
   if (batch == 0) return RONK_OK;
   const u64 mask = mul ? (((u64)1 << log_n) - 1) : ~0ULL;
   return with_field(ctx, p, g, false, [&](const auto& f) {

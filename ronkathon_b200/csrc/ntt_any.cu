@@ -110,12 +110,6 @@ anyntt_chirp_table_kernel(const F f, u64 n, u64 N, u64 w_tw, u64* __restrict__ r
   }
 }
 
-static u32 log2_ceil_u64(u64 v) {
-  u32 k = 0;
-  while (k < 63 && ((u64)1 << k) < v) k++;
-  return k;
-}
-
 // Which kernels run a transform of n points (anyntt_path, AnyNttPath in ronk_internal.h): the power-of-two transform;
 // Bluestein when its convolution of N = 2^⌈log2(2n - 1)⌉ ≤ 2^26 points divides p - 1 and n reaches the crossover; the
 // literal evaluation at n roots of unity (ronk_dft_u64's kernels) up to kAnyNttLiteralMax; else nothing.
@@ -127,9 +121,9 @@ constexpr u64 kAnyNttMin = 4080;
 
 static AnyNttPath anyntt_path(const ronk_ctx* ctx, u64 p, u64 n) {
   if ((n & (n - 1)) == 0) return AN_POW2;
-  const u32 log_N = log2_ceil_u64(2 * n - 1);
+  const u32 log_N = log2_ceil(2 * n - 1);
   const u64 min_n = ctx->tune.anyntt_min >= 0 ? (u64)ctx->tune.anyntt_min : kAnyNttMin;
-  if (log_N <= 26 && (p - 1) % ((u64)1 << log_N) == 0 && n >= min_n) return AN_BLUESTEIN;
+  if (pow2_fits(p, log_N) && n >= min_n) return AN_BLUESTEIN;
   if (n <= kAnyNttLiteralMax) return AN_LITERAL;
   return AN_NONE;
 }
@@ -178,7 +172,7 @@ static int anyntt_spectrum(ronk_ctx* ctx, u64 p, u64 g, u64 n, u32 log_N, const 
 }
 
 static int anyntt_bluestein(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int inverse) {
-  const u32 log_N = log2_ceil_u64(2 * n - 1);
+  const u32 log_N = log2_ceil(2 * n - 1);
   const u64 N = (u64)1 << log_N;
   if ((u64)an_grid(N, 1) * batch > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
   const u64* R = nullptr;
@@ -231,7 +225,7 @@ int anyntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, u64 n, u32 batch, int 
   RONK_TRY(anyntt_args(ctx, p, g, data, n, &path));
   if (batch == 0) return RONK_OK;
   switch (path) {
-    case AN_POW2: return ntt_device(ctx, p, g, data, nullptr, log2_ceil_u64(n), batch, inverse);
+    case AN_POW2: return ntt_device(ctx, p, g, data, nullptr, log2_ceil(n), batch, inverse);
     case AN_BLUESTEIN: return anyntt_bluestein(ctx, p, g, data, n, batch, inverse);
     default: return anyntt_literal(ctx, p, g, data, n, batch, inverse);
   }

@@ -402,33 +402,6 @@ __global__ void interp_sum_kernel(const F f, const u64* __restrict__ partial, u3
   out[i] = acc;
 }
 
-template <class F>
-static int poly_mul_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u64* a, size_t da, const u64* b,
-                               size_t db, u64* c) {
-  const size_t L = da + db - 1;
-  u32 log_n = 0;
-  while (((size_t)1 << log_n) < L) log_n++;
-  const bool ntt_ok = g != 0 && log_n >= 1 && log_n <= 26 && (p - 1) % ((u64)1 << log_n) == 0;
-  // NTT cost ~ 3·n·log n / 2 multiplies vs da·db for schoolbook
-  const double school = (double)da * (double)db;
-  const double viantt = 1.5 * (double)((size_t)1 << log_n) * (double)log_n + 4096.0;
-  if (!ntt_ok || school <= viantt) {
-    if (crt_mul_fits(ctx, p, g, da, db)) return crt_mul_device(ctx, p, a, da, b, db, c);  // poly_crt.cu
-    return launch(ctx, "poly_mul_schoolbook", poly_mul_schoolbook_kernel<F>, grid_for(ctx, L, 128), 128, 0, false, f, a, da, b,
-                  db, db, c, (u64)L);
-  }
-  const size_t n = (size_t)1 << log_n;
-  Frame fr(ctx);
-  u64* A = nullptr;
-  RONK_TRY(fr.take(&A, 2 * n));
-  u64* B = A + n;
-  // the zero padding of a and b and the clipping of the product to L coefficients happen inside the
-  // transforms' load / store phases (no pad-copy kernels, no final device copy)
-  RONK_TRY(ntt_device_bounded(ctx, p, g, a, da, A, n, nullptr, log_n, 0));  // Â
-  RONK_TRY(ntt_device_bounded(ctx, p, g, b, db, B, n, A, log_n, 0));        // B̂ ⊙ Â fused into the last stage
-  return ntt_device_bounded(ctx, p, g, B, n, c, L, nullptr, log_n, 1);      // back to coefficients, L of them
-}
-
 int poly_mul_schoolbook_rows(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, size_t b_stride,
                              u64 batch, u64* c) {
   const u64 total = batch * (u64)(da + db - 1);
@@ -442,7 +415,23 @@ static int poly_mul_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da,
   if (!ctx || !a || !b || !c) return set_err(ctx, RONK_EINVAL, "null argument");
   if (da == 0 || db == 0) return set_err(ctx, RONK_EINVAL, "empty polynomial (D + D2 - 1 underflows)");
   RONK_TRY(validate_modulus(ctx, p));
-  return with_field(ctx, p, g, false, [&](const auto& f) { return poly_mul_with_field(ctx, f, p, g, a, da, b, db, c); });
+  const size_t L = da + db - 1;
+  const u32 log_n = log2_ceil(L);
+  const bool ntt_ok = g != 0 && log_n >= 1 && pow2_fits(p, log_n);
+  // NTT cost ~ 3·n·log n / 2 multiplies vs da·db for schoolbook
+  const double school = (double)da * (double)db;
+  const double viantt = 1.5 * (double)((size_t)1 << log_n) * (double)log_n + 4096.0;
+  if (!ntt_ok || school <= viantt) {
+    if (crt_mul_fits(ctx, p, g, da, db)) return crt_mul_device(ctx, p, a, da, b, db, c);  // poly_crt.cu
+    return poly_mul_schoolbook_rows(ctx, p, a, da, b, db, db, 1, c);
+  }
+  const size_t n = (size_t)1 << log_n;
+  Frame fr(ctx);
+  u64* X = nullptr;
+  RONK_TRY(fr.take(&X, 2 * n));
+  // the zero padding of a and b and the clipping of the product to L coefficients happen inside the
+  // transforms' load / store phases (no pad-copy kernels, no final device copy)
+  return product_bounded(ctx, p, g, a, da, b, db, log_n, X, X + n, c, L);
 }
 
 template <bool SUB>

@@ -37,12 +37,6 @@ constexpr u64 kBatchMaxWords = (u64)1 << 40, kBatchMaxTransformWords = (u64)1 <<
 
 constexpr int PAD_THREADS = 256;
 
-static u32 log2_ceil(size_t v) {
-  u32 k = 0;
-  while (((size_t)1 << k) < v) k++;
-  return k;
-}
-
 // dst[r·N + k] = k < d ? src[r·stride + k] : 0, over total = rows·N words.
 __global__ void __launch_bounds__(PAD_THREADS)
 poly_rows_pad_kernel(const u64* __restrict__ src, u32 d, u64 stride, u32 log_n, u64 total, u64* __restrict__ dst) {
@@ -132,7 +126,7 @@ static BatchPath batch_path(const ronk_ctx* ctx, u64 p, u64 g, size_t da, size_t
   const size_t L = da + db - 1;
   const u32 log_n = log2_ceil(L);
   const bool fits = g != 0 && log_n >= 1 && L <= kCrtMulMaxLen;
-  const bool pow2 = fits && (p - 1) % ((u64)1 << log_n) == 0;
+  const bool pow2 = fits && pow2_fits(p, log_n);
   if (!fits) return BP_SCHOOL;
   const int forced = ctx->tune.poly_batch_path;
   if (forced == 1) return BP_SCHOOL;

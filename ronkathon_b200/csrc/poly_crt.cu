@@ -45,22 +45,35 @@ crt_combine_kernel(const F f, const CrtConsts k, const u64* __restrict__ C, size
 constexpr u64 kCrtMulMin[kCrtPrimes] = {(u64)1 << 16, (u64)1 << 20, (u64)1 << 20};
 constexpr size_t kCrtMulShortMin[kCrtPrimes] = {256, 512, 1024};
 
-static u32 log2_ceil(size_t v) {
-  u32 k = 0;
-  while (((size_t)1 << k) < v) k++;
-  return k;
-}
-
 bool crt_mul_fits(const ronk_ctx* ctx, u64 p, u64 g, size_t da, size_t db) {
   const size_t L = da + db - 1;
   if (g == 0 || L > kCrtMulMaxLen) return false;
-  if ((p - 1) % ((u64)1 << log2_ceil(L)) == 0) return false;  // the direct transform fits
-  const u64 work = (u64)da * (u64)db;                         // da, db ≤ L ≤ 2^26: no overflow
+  if (pow2_fits(p, log2_ceil(L))) return false;  // the direct transform fits
+  const u64 work = (u64)da * (u64)db;             // da, db ≤ L ≤ 2^26: no overflow
   const long long forced = ctx->tune.crt_mul_min;
   if (forced >= 0) return work >= (u64)forced;
   const size_t m = std::min(da, db);
   const int k = crt_prime_count(p, m);
   return work >= kCrtMulMin[k - 1] && m >= kCrtMulShortMin[k - 1];
+}
+
+static int crt_reduce(ronk_ctx* ctx, u64 q, const u64* a, size_t na, u64* ra, const u64* b, size_t nb, u64* rb) {
+  return launch(ctx, "crt_reduce", crt_reduce_kernel, grid_for(ctx, std::max(na, nb), CRT_THREADS), CRT_THREADS, 0, false, q,
+                a, na, ra, b, nb, rb);
+}
+
+// c[0, len) mod p from the K residue vectors C[i·len, (i + 1)·len), i < K.
+static int crt_combine(ronk_ctx* ctx, u64 p, int K, const u64* C, size_t len, u64* c) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    const CrtConsts k = crt_consts(f);
+    const int grid = grid_for(ctx, len, CRT_THREADS);
+    switch (K) {
+      case 1: return launch(ctx, "crt_combine", crt_combine_kernel<F, 1>, grid, CRT_THREADS, 0, false, f, k, C, len, c);
+      case 2: return launch(ctx, "crt_combine", crt_combine_kernel<F, 2>, grid, CRT_THREADS, 0, false, f, k, C, len, c);
+      default: return launch(ctx, "crt_combine", crt_combine_kernel<F, 3>, grid, CRT_THREADS, 0, false, f, k, C, len, c);
+    }
+  });
 }
 
 // Per auxiliary prime q_i: [reduce a into B and b into C_i when q_i < p], Â into A, B̂ ⊙ Â into B, the inverse into C_i
@@ -76,29 +89,17 @@ int crt_mul_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, 
   u64* B = A + n;
   u64* C = B + n;
   for (int i = 0; i < K; i++) {
-    const u64 q = kCrtQ[i], g = kCrtG[i];
+    const u64 q = kCrtQ[i];
     u64* Ci = C + (size_t)i * L;
     const u64 *sa = a, *sb = b;
     if (q < p) {
-      RONK_TRY(launch(ctx, "crt_reduce", crt_reduce_kernel, grid_for(ctx, std::max(da, db), CRT_THREADS), CRT_THREADS, 0, false,
-                      q, a, da, B, b, db, Ci));
+      RONK_TRY(crt_reduce(ctx, q, a, da, B, b, db, Ci));
       sa = B;
       sb = Ci;
     }
-    RONK_TRY(ntt_device_bounded(ctx, q, g, sa, da, A, n, nullptr, log_n, 0));  // Â
-    RONK_TRY(ntt_device_bounded(ctx, q, g, sb, db, B, n, A, log_n, 0));        // B̂ ⊙ Â
-    RONK_TRY(ntt_device_bounded(ctx, q, g, B, n, Ci, L, nullptr, log_n, 1));   // residues mod q_i, L of them
+    RONK_TRY(product_bounded(ctx, q, kCrtG[i], sa, da, sb, db, log_n, A, B, Ci, L));  // residues mod q_i, L of them
   }
-  return with_field(ctx, p, 0, false, [&](const auto& f) {
-    using F = std::decay_t<decltype(f)>;
-    const CrtConsts k = crt_consts(f);
-    const int grid = grid_for(ctx, L, CRT_THREADS);
-    switch (K) {
-      case 1: return launch(ctx, "crt_combine", crt_combine_kernel<F, 1>, grid, CRT_THREADS, 0, false, f, k, C, L, c);
-      case 2: return launch(ctx, "crt_combine", crt_combine_kernel<F, 2>, grid, CRT_THREADS, 0, false, f, k, C, L, c);
-      default: return launch(ctx, "crt_combine", crt_combine_kernel<F, 3>, grid, CRT_THREADS, 0, false, f, k, C, L, c);
-    }
-  });
+  return crt_combine(ctx, p, K, C, L, c);
 }
 
 // The same path over `batch` contiguous rows (ronk_poly_mul_batch_u64): one crt_reduce over the flat batch·da and
@@ -130,23 +131,13 @@ int crt_mul_rows_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64
         RONK_TRY(fr.take(&ra, na));
         RONK_TRY(fr.take(&rb, nb));
       }
-      RONK_TRY(launch(ctx, "crt_reduce", crt_reduce_kernel, grid_for(ctx, std::max(na, nb), CRT_THREADS), CRT_THREADS, 0, false,
-                      q, a, na, ra, b, nb, rb));
+      RONK_TRY(crt_reduce(ctx, q, a, na, ra, b, nb, rb));
       sa = ra;
       sb = rb;
     }
     RONK_TRY(poly_mul_rows_pow2(ctx, q, g, sa, da, sb, db, b_shared, batch, C + (size_t)i * total));
   }
-  return with_field(ctx, p, 0, false, [&](const auto& f) {
-    using F = std::decay_t<decltype(f)>;
-    const CrtConsts k = crt_consts(f);
-    const int grid = grid_for(ctx, total, CRT_THREADS);
-    switch (K) {
-      case 1: return launch(ctx, "crt_combine", crt_combine_kernel<F, 1>, grid, CRT_THREADS, 0, false, f, k, C, total, c);
-      case 2: return launch(ctx, "crt_combine", crt_combine_kernel<F, 2>, grid, CRT_THREADS, 0, false, f, k, C, total, c);
-      default: return launch(ctx, "crt_combine", crt_combine_kernel<F, 3>, grid, CRT_THREADS, 0, false, f, k, C, total, c);
-    }
-  });
+  return crt_combine(ctx, p, K, C, total, c);
 }
 
 }  // namespace ronk

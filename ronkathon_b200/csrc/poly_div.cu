@@ -15,8 +15,7 @@
 namespace ronk {
 
 // dst[i] = i < n ? src[last - i] : 0, i < dst_len: reverses, truncates and zero-fills in one pass
-__global__ void divrem_reverse_kernel(const u64* __restrict__ src, size_t last, size_t n, u64* __restrict__ dst,
-                                      size_t dst_len) {
+__global__ void reverse_kernel(const u64* __restrict__ src, size_t last, size_t n, u64* __restrict__ dst, size_t dst_len) {
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dst_len; i += stride)
     dst[i] = (i < n) ? src[last - i] : 0ULL;
@@ -45,12 +44,6 @@ __global__ void divrem_fold_kernel(const F f, const u64* __restrict__ src, size_
   }
 }
 
-static u32 log2_ceil(size_t v) {  // v ≤ 2^63
-  u32 k = 0;
-  while (k < 63 && ((size_t)1 << k) < v) k++;
-  return k;
-}
-
 // Transform sizes (log2) of the plan: the quotient product (also the largest Newton step) and the remainder product.
 // The remainder needs only b·q mod x^(db-1).  A quotient at least that long is cut to its low db - 1 words, like b,
 // and the product runs without wrap (2(db-1) - 1 points); a shorter one keeps every word and the product is taken mod
@@ -66,7 +59,7 @@ bool divrem_newton_fits(u64 p, u64 g, size_t da, size_t db) {
   u32 lq, lr;
   divrem_newton_sizes(da, db, &lq, &lr);
   const u32 lmax = std::max(lq, lr);
-  return lmax <= 26 && (p - 1) % ((u64)1 << lmax) == 0;
+  return pow2_fits(p, lmax);
 }
 
 template <class F>
@@ -75,9 +68,8 @@ static int fold(ronk_ctx* ctx, const F& f, const u64* src, size_t len, size_t n,
                 dst_len);
 }
 
-static int reverse(ronk_ctx* ctx, const u64* src, size_t last, size_t n, u64* dst, size_t dst_len) {
-  return launch(ctx, "divrem_reverse", divrem_reverse_kernel, grid_for(ctx, dst_len, 256), 256, 0, false, src, last, n, dst,
-                dst_len);
+int reverse_words(ronk_ctx* ctx, const char* name, const u64* src, size_t last, size_t n, u64* dst, size_t dst_len) {
+  return launch(ctx, name, reverse_kernel, grid_for(ctx, dst_len, 256), 256, 0, false, src, last, n, dst, dst_len);
 }
 
 // G = hr^-1 mod x^L by Newton doubling, hr of hl ≤ L words with hr[0]^-1 = g1: g_2t = g_t·(2 - hr·g_t) mod x^2t on
@@ -119,14 +111,12 @@ static int divrem_newton_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, con
   u64* G = Y + nx;
   u64* AR = G + L;
   u64* HR = AR + L;
-  RONK_TRY(reverse(ctx, a, da - 1, L, AR, L));
-  RONK_TRY(reverse(ctx, b, db - 1, hl, HR, hl));
+  RONK_TRY(reverse_words(ctx, "divrem_reverse", a, da - 1, L, AR, L));
+  RONK_TRY(reverse_words(ctx, "divrem_reverse", b, db - 1, hl, HR, hl));
   RONK_TRY(newton_inverse(ctx, f, p, g, HR, hl, L, h_powmod(top, p - 2, p), G, X, Y));  // g_1 = b[db-1]^-1
   // rev(q) = ar·inv mod x^L (nq ≥ 2L - 1: no wrap into the low L words), into AR, then reversed into q
-  RONK_TRY(ntt_device_bounded(ctx, p, g, AR, L, X, nq, nullptr, lq, 0));
-  RONK_TRY(ntt_device_bounded(ctx, p, g, G, L, Y, nq, X, lq, 0));
-  RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nq, AR, L, nullptr, lq, 1));
-  RONK_TRY(reverse(ctx, AR, L - 1, L, q, da));
+  RONK_TRY(product_bounded(ctx, p, g, AR, L, G, L, lq, X, Y, AR, L));
+  RONK_TRY(reverse_words(ctx, "divrem_reverse", AR, L - 1, L, q, da));
   const size_t rw = db - 1;  // remainder words
   if (rw == 0) {
     RONK_CUDA(ctx, cudaMemsetAsync(r, 0, da * sizeof(u64), ctx->stream));
@@ -134,18 +124,14 @@ static int divrem_newton_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, con
   }
   const u64* A = a;
   if (L >= rw) {  // low product: (b mod x^rw)·(q mod x^rw), nr ≥ 2·rw - 1
-    RONK_TRY(ntt_device_bounded(ctx, p, g, b, rw, X, nr, nullptr, lr, 0));
-    RONK_TRY(ntt_device_bounded(ctx, p, g, q, rw, Y, nr, X, lr, 0));
-    RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nr, Y, rw, nullptr, lr, 1));
+    RONK_TRY(product_bounded(ctx, p, g, b, rw, q, rw, lr, X, Y, Y, rw));
   } else {  // b·q mod x^nr - 1, nr ≥ rw > L (q needs no fold; da < 2·rw, so every fold adds at most two terms)
     if (db > nr) {
       RONK_TRY(fold(ctx, f, b, db, nr, X, nr));
-      RONK_TRY(ntt_device_bounded(ctx, p, g, X, nr, X, nr, nullptr, lr, 0));
+      RONK_TRY(product_bounded(ctx, p, g, X, nr, q, L, lr, X, Y, Y, rw));
     } else {
-      RONK_TRY(ntt_device_bounded(ctx, p, g, b, db, X, nr, nullptr, lr, 0));
+      RONK_TRY(product_bounded(ctx, p, g, b, db, q, L, lr, X, Y, Y, rw));
     }
-    RONK_TRY(ntt_device_bounded(ctx, p, g, q, L, Y, nr, X, lr, 0));
-    RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nr, Y, rw, nullptr, lr, 1));
     if (da > nr) {
       RONK_TRY(fold(ctx, f, a, da, nr, X, rw));
       A = X;

@@ -35,12 +35,6 @@ RONK_HD size_t node_deg(size_t k, u32 j, size_t i) {
   return lo >= k ? 0 : (k - lo < w ? k - lo : w);
 }
 
-static u32 log2_ceil(size_t v) {
-  u32 k = 0;
-  while (k < 63 && ((size_t)1 << k) < v) k++;
-  return k;
-}
-
 // The product of the 2^lb leaves of subtree blockIdx.x, schoolbook level by level in shared memory (nodes of level j
 // at stride 2^j + 1), to out[blockIdx.x·(2^lb + 1) …].  With cs: also the interpolation sums r (leaf r = cs[i], level
 // j at stride 2^j) to rout[blockIdx.x·2^lb …].
@@ -130,12 +124,6 @@ __global__ void tree_extract_kernel(const u64* __restrict__ A, const u64* __rest
   }
 }
 
-// dst[i] = i < n ? src[last - i] : 0, i < dst_len
-__global__ void tree_reverse_kernel(const u64* __restrict__ src, size_t last, size_t n, u64* __restrict__ dst, size_t dst_len) {
-  const size_t step = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dst_len; i += step) dst[i] = i < n ? src[last - i] : 0ULL;
-}
-
 // out[i] = (i + 1)·M[i + 1], i < k
 template <class F>
 __global__ void tree_deriv_kernel(const F f, const u64* __restrict__ M, size_t k, u64* __restrict__ out) {
@@ -204,10 +192,6 @@ static int spread(ronk_ctx* ctx, const u64* src, size_t stride, size_t len, u32 
                 A, B);
 }
 
-static int reverse(ronk_ctx* ctx, const u64* src, size_t last, size_t n, u64* dst, size_t dst_len) {
-  return launch(ctx, "tree_reverse", tree_reverse_kernel, grid_for(ctx, dst_len, 256), 256, 0, false, src, last, n, dst, dst_len);
-}
-
 // Levels lb … K of the product tree (T[0], T[1] scratch).
 template <class F>
 static int tree_build(ronk_ctx* ctx, const F& f, u64 p, u64 g, const Tree& t, const u64* xs) {
@@ -242,13 +226,11 @@ static int tree_down(ronk_ctx* ctx, const F& f, u64 p, u64 g, const Tree& t, con
   u64* G = Y + nq;
   u64* FR = G + d;
   u64* HR = FR + d;
-  RONK_TRY(reverse(ctx, t.M + t.off[t.K], k, hl, HR, hl));  // rev_k(M) mod y^hl; M monic: HR[0] = 1
+  RONK_TRY(reverse_words(ctx, "tree_reverse", t.M + t.off[t.K], k, hl, HR, hl));  // rev_k(M) mod y^hl; M monic: HR[0] = 1
   RONK_TRY(newton_inverse_device(ctx, p, g, HR, hl, d, 1, G, X, Y));
-  RONK_TRY(reverse(ctx, c, d - 1, d, FR, d));
-  RONK_TRY(ntt_device_bounded(ctx, p, g, FR, d, X, nq, nullptr, lq, 0));
-  RONK_TRY(ntt_device_bounded(ctx, p, g, G, d, Y, nq, X, lq, 0));
-  RONK_TRY(ntt_device_bounded(ctx, p, g, Y, nq, FR, d, nullptr, lq, 1));
-  RONK_TRY(reverse(ctx, FR, d - 1, std::min(d, k), R, t.N));
+  RONK_TRY(reverse_words(ctx, "tree_reverse", c, d - 1, d, FR, d));
+  RONK_TRY(product_bounded(ctx, p, g, FR, d, G, d, lq, X, Y, FR, d));
+  RONK_TRY(reverse_words(ctx, "tree_reverse", FR, d - 1, std::min(d, k), R, t.N));
   for (u32 j = t.K; j-- > t.lb;) {  // parents at level j + 1
     const u32 ld = j + 1;
     const size_t w = (size_t)1 << j, P = t.N >> ld;
@@ -271,7 +253,7 @@ bool tree_fits(u64 p, u64 g, size_t k, size_t d) {
   const u32 K = log2_ceil(k);
   u32 lmax = K > TREE_B ? K : 0;
   if (d) lmax = std::max(lmax, std::max<u32>(1, log2_ceil(2 * d - 1)));
-  return lmax <= 26 && (p - 1) % ((u64)1 << lmax) == 0;
+  return pow2_fits(p, lmax);
 }
 
 int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out) {

@@ -383,6 +383,16 @@ inline int stage_out(ronk_ctx* ctx, int rc, const Staged (&r)[N]) {
 // Whether the nx words at x and the ny words at y share a word.
 inline bool overlaps(const u64* x, size_t nx, const u64* y, size_t ny) { return nx && ny && x < y + ny && y < x + nx; }
 
+// ⌈log2 v⌉, capped at 63 (v ≤ 1 gives 0).
+inline u32 log2_ceil(u64 v) {
+  u32 k = 0;
+  while (k < 63 && ((u64)1 << k) < v) k++;
+  return k;
+}
+
+// Whether the power-of-two transforms take 2^log_n points over p: log_n ≤ 26 and 2^log_n divides p - 1.
+inline bool pow2_fits(u64 p, u32 log_n) { return log_n <= 26 && (p - 1) % ((u64)1 << log_n) == 0; }
+
 int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out);  // ntt.cu
 int validate_modulus(ronk_ctx* ctx, u64 p);                                       // field_ops.cu
 
@@ -405,6 +415,14 @@ int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n
 int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst, const u64* mul, u32 log_n, u32 batch);
 int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len, u64* dst, u64 dst_len, const u64* mul,
                        u32 log_n, int inverse);
+// out[0, out_len) = a·b mod x^n - 1, n = 2^log_n, by three bounded transforms: a[0, la) → X, b[0, lb) → Y ⊙ X, the
+// inverse of Y → out.  X and Y hold n words each.  a may be X, and out may be a, b or Y: a transform may run in place,
+// and a and b are read by the first two transforms only.  Stream-ordered.
+int product_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* a, u64 la, const u64* b, u64 lb, u32 log_n, u64* X, u64* Y,
+                    u64* out, u64 out_len);
+// poly_div.cu: dst[i] = i < n ? src[last - i] : 0 for i < dst_len (reverses, truncates and zero-fills in one pass), one
+// launch profiled as `name`.
+int reverse_words(ronk_ctx* ctx, const char* name, const u64* src, size_t last, size_t n, u64* dst, size_t dst_len);
 // The single-tile plan of 2^log_n points (log_n ≤ 13): per-round twiddle tables (forward, inverse) and n^-1, twiddle form.
 int ntt_single_tables(ronk_ctx* ctx, u64 p, u64 g, u32 log_n, const u64** fwd, const u64** inv, u64* scale_inv);
 // poly.cu: nodes[i] = ω_n^i (plain residues), n ≤ 2^31 - 1; out[i] = Σ_j c_j xs[i]^j, one CTA per point
