@@ -64,6 +64,10 @@ extern "C" {
   pub fn ronk_dft_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, input: *const u64, n: u64, out: *mut u64) -> c_int;
   pub fn ronk_ntt_any_u64(ctx: *mut ronk_ctx, p: u64, g: u64, data: *mut u64, n: u64, batch: u32, inverse: c_int) -> c_int;
   pub fn ronk_ntt_any_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, host_data: *mut u64, n: u64, batch: u32, inverse: c_int) -> c_int;
+  pub fn ronk_ntt_coset_u64(ctx: *mut ronk_ctx, p: u64, g: u64, data: *mut u64, log_n: u32, batch: u32, shift: u64, inverse: c_int) -> c_int;
+  pub fn ronk_ntt_coset_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, host_data: *mut u64, log_n: u32, batch: u32, shift: u64, inverse: c_int) -> c_int;
+  pub fn ronk_poly_lde_u64(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, d: usize, log_n: u32, shift: u64, batch: u32, out: *mut u64) -> c_int;
+  pub fn ronk_poly_lde_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, d: usize, log_n: u32, shift: u64, batch: u32, out: *mut u64) -> c_int;
 
   // Polynomial arithmetic (src/polynomial/arithmetic.rs, mod.rs:133-225, :382-415)
   pub fn ronk_poly_mul_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, c: *mut u64) -> c_int;

@@ -111,6 +111,36 @@ int ronk_ntt_u64_host_wait(ronk_ctx *ctx, int slot);
 /* Forward transform whose last stage also multiplies point-wise by `mul` (same shape, natural
  * order): data[k] = NTT(data)[k] * mul[k].  The fused form of the evaluate→multiply step. */
 int ronk_ntt_mul_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *data, const uint64_t *mul, uint32_t log_n, uint32_t batch);
+/* Coset transforms: in place, `batch` contiguous transforms of n = 2^log_n points on the coset s·H_n of the subgroup
+ * H_n = {ω_n^k}, natural order, ω_n as for ronk_ntt_u64, s = `shift`:
+ *   forward  X[k] = Σ_j a_j (s·ω_n^k)^j;   inverse: the a with those X, a_j = s^-j · n^-1 Σ_k X_k ω_n^(-jk).
+ * - Any s in F_p* (elements of H_n included).  s = 1 gives exactly ronk_ntt_u64's words, through its own path.
+ *   log_n = 0 is the identity.  Residues are canonical.
+ * - Errors: those of ronk_ntt_u64 (RONK_EINVAL if 2^log_n does not divide p - 1, for a null pointer, g == 0 or g >= p;
+ *   RONK_EUNSUPPORTED if log_n > 26), and RONK_EINVAL for s == 0 or s >= p.  batch == 0 does nothing.  Every check is
+ *   made and all scratch (RONK_ENOMEM) is taken before anything is enqueued; on failure nothing is written.
+ * - Kernels: the factor s^j (forward) or s^-j (inverse) is applied to the word at natural index j of its transform in
+ *   the load of the first pass or the store of the last, so the transform moves the bytes of the plain one.  One small
+ *   launch per call builds the factor tables: s^±i for i < 2^h and s^±(i·2^h) for i < 2^(log_n - h), h = ⌈log_n / 2⌉.
+ *   n ≤ 2^13: the single-tile kernel; Goldilocks with g = 7 at 2^21 … 2^24: the three 256-point-tile passes; every
+ *   other size and field: the generic two-pass tile kernels.  The cluster, split and interleaved kernels of
+ *   ronk_ntt_u64 (Goldilocks 2^16 … 2^20, 2^25, 2^26) are not used, whatever the context's transform switches say.
+ * - Scratch: the factor tables, 2^h + 2^(log_n - h) words (≤ 16 Ki), and for n > 2^13 the transform's workspace of
+ *   batch·n words.
+ * - The device variant is asynchronous on the context's stream; the _host variant stages in and out and synchronises. */
+int ronk_ntt_coset_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *data, uint32_t log_n, uint32_t batch, uint64_t shift, int inverse);
+int ronk_ntt_coset_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, uint64_t *host_data, uint32_t log_n, uint32_t batch, uint64_t shift, int inverse);
+/* Low-degree extension: row r of coeffs (d words each, 1 ≤ d ≤ N = 2^log_n) evaluated on shift·H_N,
+ *   out[r][k] = Σ_{j<d} coeffs[r][j] (shift·ω_N^k)^j, out is batch × N words.
+ * - One launch copies the rows into out zero-extended to N words (poly_rows_pad_kernel), then the forward coset
+ *   transform of ronk_ntt_coset_u64 runs in place on out (ronk_ntt_u64's transform for shift = 1).  Scratch: that of the
+ *   transform, nothing more.
+ * - Errors: those of ronk_ntt_coset_u64 for (p, g, log_n, shift), and RONK_EINVAL for a null coeffs, d == 0, d > N or
+ *   an out that overlaps coeffs; RONK_EUNSUPPORTED for batch·N > 2^32 words.  batch == 0 does nothing.  Every check is
+ *   made and all scratch is taken before anything is enqueued; on failure nothing is written.  coeffs is only read.
+ * - The device variant is asynchronous on the context's stream; the _host variant stages in and out and synchronises. */
+int ronk_poly_lde_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t d, uint32_t log_n, uint64_t shift, uint32_t batch, uint64_t *out);
+int ronk_poly_lde_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t d, uint32_t log_n, uint64_t shift, uint32_t batch, uint64_t *out);
 /* Polynomial::dft — src/polynomial/mod.rs:240-258.  Any n | p-1 (O(n²)); out must not alias in. */
 int ronk_dft_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *in, uint64_t n, uint64_t *out);
 int ronk_dft_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *in, uint64_t n, uint64_t *out);

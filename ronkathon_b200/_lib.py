@@ -59,6 +59,10 @@ SIGNATURES = {
     "ronk_dft_u64_host": (i32, [vp, u64, u64, vp, u64, vp]),
     "ronk_ntt_any_u64": (i32, [vp, u64, u64, vp, u64, u32, i32]),
     "ronk_ntt_any_u64_host": (i32, [vp, u64, u64, vp, u64, u32, i32]),
+    "ronk_ntt_coset_u64": (i32, [vp, u64, u64, vp, u32, u32, u64, i32]),
+    "ronk_ntt_coset_u64_host": (i32, [vp, u64, u64, vp, u32, u32, u64, i32]),
+    "ronk_poly_lde_u64": (i32, [vp, u64, u64, vp, sz, u32, u64, u32, vp]),
+    "ronk_poly_lde_u64_host": (i32, [vp, u64, u64, vp, sz, u32, u64, u32, vp]),
     "ronk_poly_mul_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_mul_u64_host": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_mul_batch_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, i32, u32, vp]),

@@ -102,23 +102,29 @@ static int interpass_table(ronk_ctx* ctx, const F& f, NttPlan& pl, bool inverse,
   return RONK_OK;
 }
 
-template <class F, int MODE, bool INV, int NTHR, int MINB, bool BOUNDED, bool FMUL>
+template <class F, int MODE, bool INV, int NTHR, int MINB, bool BOUNDED, bool FMUL, bool COSET = false>
 static int launch_tile_nb(ronk_ctx* ctx, const F& f, const NttTileArgs& A0, u32 tiles, const char* name) {
   NttTileArgs A = A0;
   if (MODE == MODE_PASS1) A.prefetch_dist = (u32)ctx->tune.pf_dist * (u32)ctx->sm_count * (u32)MINB;
   const size_t smem = ((size_t)1 << A.tile_log) * sizeof(u64) + (size_t)A.tw_words * sizeof(u64) + 16;
   // the attribute is per device: set once per (context, instantiation)
-  RONK_TRY(ensure_smem_attr(ctx, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL>, 226 * 1024));
+  RONK_TRY(ensure_smem_attr(ctx, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL, COSET>, 226 * 1024));
   // pass 2 directly follows its pass 1 on the stream and may start early.  That helps launch-bound jobs (2^14…2^18) and
   // hurts a 2^24 transform (the waiting CTAs start in lockstep), so only small jobs take it
   const bool pdl = MODE == MODE_PASS2 && ctx->tune.pdl && (((u64)tiles << A.tile_log) <= ((u64)1 << 21));
-  return launch(ctx, name, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL>, tiles, NTHR, smem, pdl, f, A);
+  return launch(ctx, name, ntt_tile_kernel<F, MODE, INV, NTHR, MINB, BOUNDED, FMUL, COSET>, tiles, NTHR, smem, pdl, f, A);
 }
 
 // The bounded instantiation exists only where poly_mul needs it: a zero-padded SOURCE enters through
 // pass 1 / a single-pass tile, a clipped DESTINATION leaves through pass 2 / a single-pass tile.
 template <class F, int MODE, bool INV, int NTHR, int MINB>
 static int launch_tile_n(ronk_ctx* ctx, const F& f, const NttTileArgs& A, u32 tiles, const char* name) {
+  // a coset transform's hooked pass (forward: the first, inverse: the last) has an instantiation of its own; the other
+  // pass is the plain one
+  constexpr bool can_coset = MODE == MODE_SINGLE || (MODE == MODE_PASS1) != INV;
+  if constexpr (can_coset) {
+    if (A.coset_lo) return launch_tile_nb<F, MODE, INV, NTHR, MINB, false, false, true>(ctx, f, A, tiles, name);
+  }
   const bool bounded = (MODE != MODE_PASS2 && A.src_len != NTT_UNBOUNDED) || (MODE != MODE_PASS1 && A.dst_len != NTT_UNBOUNDED);
   // the fused point-wise multiply of pass 2 (forward transforms of poly_mul) has its own instantiation too
   constexpr bool can_fmul = MODE == MODE_PASS2 && !INV && ((RONK_STORE_V0_MASK >> MODE_PASS2) & 1);
@@ -159,7 +165,7 @@ static int launch12(ronk_ctx* ctx, const GoldilocksField& f, const NttTileArgs& 
 template <class F, int MODE, bool INV>
 static int launch_tile(ronk_ctx* ctx, const F& f, const NttTileArgs& A, u32 tiles, const char* name) {
   if constexpr (std::is_same<F, GoldilocksField>::value && MODE != MODE_SINGLE) {
-    if (ctx->tune.fast12 && ntt12_applicable(A, MODE) && !(INV && (A.flags & NTT_FLAG_MUL)))
+    if (ctx->tune.fast12 && !A.coset_lo && ntt12_applicable(A, MODE) && !(INV && (A.flags & NTT_FLAG_MUL)))
       return launch12<MODE, INV>(ctx, f, A, tiles, name);
   }
   const u32 groups = (1u << A.tile_log) / 16;
@@ -170,12 +176,12 @@ static int launch_tile(ronk_ctx* ctx, const F& f, const NttTileArgs& A, u32 tile
 }
 
 // ---- transforms as passes of 256-point tiles (ntt3_kernel.cuh): n = 2^24 (three passes) and n = 2^16 (two) -------
-template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int NG, int LI = 0>
+template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int NG, int LI = 0, bool COSET = false>
 static int launch3_ng(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* name, bool dependent, unsigned tiles) {
-  return launch(ctx, name, ntt3_kernel<F, PASS, INV, LOGN, BOUNDED, NG, LI>, tiles, N3_THREADS * (2 / NG), 0,
+  return launch(ctx, name, ntt3_kernel<F, PASS, INV, LOGN, BOUNDED, NG, LI, COSET>, tiles, N3_THREADS * (2 / NG), 0,
                 dependent && ctx->tune.ntt3_pdl, f, A);
 }
-template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int LI = 0>
+template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int LI = 0, bool COSET = false>
 static int launch3(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* name, bool dependent) {
   const unsigned tiles = A.batch * (LOGN >= 21 ? (1u << (LOGN - 12)) : LOGN == 20 ? 256u : 16u);
   // a grid that leaves most warp slots empty runs one radix-16 group per thread (256 threads per tile): a single
@@ -184,7 +190,7 @@ static int launch3(ronk_ctx* ctx, const F& f, const Ntt3Args& A, const char* nam
     if (tiles < (unsigned)ctx->tune.ntt3_ng1_tiles * (unsigned)ctx->sm_count)
       return launch3_ng<F, PASS, INV, LOGN, BOUNDED, 1, LI>(ctx, f, A, name, dependent, tiles);
   }
-  return launch3_ng<F, PASS, INV, LOGN, BOUNDED, 2, LI>(ctx, f, A, name, dependent, tiles);
+  return launch3_ng<F, PASS, INV, LOGN, BOUNDED, 2, LI, COSET>(ctx, f, A, name, dependent, tiles);
 }
 
 // pass C of the 2^20-point transform (ntt3c_kernel): one thread per (transform, k2)
@@ -283,10 +289,13 @@ static int run_ntt16_cluster(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, 
 // LI > 0: a SPLIT transform n = 2^LI·2^LOGN (2^17 … 2^19 over 2^16, 2^25 / 2^26 over 2^24): `outer` is the n-point plan (its
 // two-level tables feed the first pass), pl the 2^LOGN-point plan of the 2^LI·batch sub-transforms; ntt3p_kernel runs
 // first (src → data, in place when they coincide) and the last pass interleaves the sub-transforms' outputs.
-template <class F, bool INV, int LOGN, bool BOUNDED, int LI = 0>
+// COSET (2^21 … 2^24, unbounded, no multiplier): `coset` holds the two coset tables of run_ntt; pass 1 (forward) or
+// pass 3 (inverse) applies the factor, and every pass's profile name carries "_coset".
+template <class F, bool INV, int LOGN, bool BOUNDED, int LI = 0, bool COSET = false>
 static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64* src, const u64* mul, u32 batch,
-                    u64 src_len, u64 dst_len, u64 mul_mask = ~0ULL, const NttPlan* outer = nullptr) {
+                    u64 src_len, u64 dst_len, u64 mul_mask = ~0ULL, const NttPlan* outer = nullptr, const u64* coset = nullptr) {
   static_assert(LI == 0 || ((LOGN == 16 || LOGN == 24) && !BOUNDED), "split transforms: over 2^16 or 2^24, unbounded");
+  static_assert(!COSET || (LI == 0 && !BOUNDED && LOGN >= 21), "coset transforms: 2^21 … 2^24, unbounded");
   const int d = INV ? 1 : 0;
   const u64 n = (u64)1 << LOGN;
   RONK_TRY((ntt3_tables<F, INV>(ctx, f, pl, LOGN)));
@@ -333,6 +342,7 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
   A.mul_mask = mul_mask;
   A.src = src;
   A.dst = ws;
+  if constexpr (COSET) A.coset = coset;
   if constexpr (LOGN == 20) {
     // sixteen interleaved 2^16-point transforms + one radix-16 pass (ntt3_kernel.cuh): A1 src → data (identical views, so
     // src == data is fine), A2 data → workspace, C workspace → data.  A.tw_hi = ω_n^(1024 y): the plan's 10 / 10 split.
@@ -348,15 +358,18 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
     return launch3c<F, INV>(ctx, f, A, INV ? "intt3_c" : "ntt3_c");
   } else {
     if constexpr (LOGN >= 21) {
-      RONK_TRY((launch3<F, 1, INV, LOGN, BOUNDED>(ctx, f, A, INV ? "intt3_pass1" : "ntt3_pass1", false)));
+      const char* name = COSET ? (INV ? "intt3_pass1_coset" : "ntt3_pass1_coset") : (INV ? "intt3_pass1" : "ntt3_pass1");
+      RONK_TRY((launch3<F, 1, INV, LOGN, BOUNDED, 0, COSET && !INV>(ctx, f, A, name, false)));
       A.src = ws;
     }
-    RONK_TRY((launch3<F, 2, INV, LOGN, BOUNDED && LOGN == 16>(ctx, f, A, INV ? "intt3_pass2" : "ntt3_pass2", LOGN >= 21)));
+    const char* name2 = COSET ? (INV ? "intt3_pass2_coset" : "ntt3_pass2_coset") : (INV ? "intt3_pass2" : "ntt3_pass2");
+    RONK_TRY((launch3<F, 2, INV, LOGN, BOUNDED && LOGN == 16>(ctx, f, A, name2, LOGN >= 21)));
     A.src = ws;
     A.dst = data;
     A.mul_src = mul;
     A.flags = mul ? NTT_FLAG_MUL : 0;
-    return launch3<F, 3, INV, LOGN, BOUNDED, LI>(ctx, f, A, INV ? "intt3_pass3" : "ntt3_pass3", true);
+    const char* name3 = COSET ? (INV ? "intt3_pass3_coset" : "ntt3_pass3_coset") : (INV ? "intt3_pass3" : "ntt3_pass3");
+    return launch3<F, 3, INV, LOGN, BOUNDED, LI, COSET && INV>(ctx, f, A, name3, true);
   }
 }
 
@@ -377,11 +390,16 @@ static int plan_for(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, NttPlan*
 // src == nullptr: in place.  Otherwise (batch == 1) the transform reads src[0, src_len) zero-extended to n
 // words and writes data[0, dst_len): the zero padding of poly_mul's operands and the clipping of its
 // result happen inside the load / store phases instead of in separate copy kernels.
+// coset != nullptr: a coset transform, in place, unbounded, without multiplier.  `coset` holds c^i for i < 2^h, then
+// c^(i·2^h) for i < 2^(log_n - h), twiddle form, h = ⌈log_n / 2⌉ (c = s forward, s^-1 inverse).  It takes the
+// single-tile kernel or the generic pass pair, and the 256-point-tile passes at 2^21 … 2^24 for Goldilocks with g = 7,
+// whatever the context's transform switches say; every launch's profile name carries "_coset".
 template <class F, bool INV>
 static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64* mul, u32 batch,
                    const u64* src = nullptr, u64 src_len = NTT_UNBOUNDED, u64 dst_len = NTT_UNBOUNDED,
-                   u64 mul_mask = ~0ULL) {
+                   u64 mul_mask = ~0ULL, const u64* coset = nullptr) {
   const u32 log_n = pl.log_n;
+  const u32 coset_h = (log_n + 1) / 2;
   u64 tiles = 0;
   if (!src) src = data;
   if (src_len >= ((u64)1 << log_n)) src_len = NTT_UNBOUNDED;
@@ -394,11 +412,25 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
     A.src_len = src_len;
     A.dst_len = dst_len;
     A.mul_mask = mul_mask;
+    if (coset) {
+      A.coset_lo = coset;
+      A.coset_hi = coset + ((size_t)1 << coset_h);
+      A.coset_h = coset_h;
+    }
     if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
-    return launch_tile<F, MODE_SINGLE, INV>(ctx, f, A, (u32)tiles, INV ? "intt_single" : "ntt_single");
+    const char* name = coset ? (INV ? "intt_single_coset" : "ntt_single_coset") : (INV ? "intt_single" : "ntt_single");
+    return launch_tile<F, MODE_SINGLE, INV>(ctx, f, A, (u32)tiles, name);
   }
   if constexpr (std::is_same<F, GoldilocksField>::value) {
-    if (ctx->tune.ntt3 && !(INV && mul)) {   // mul_mask: one multiplier word per output (~0) or a shared n-word one (n - 1)
+    if (coset) {
+      switch (log_n) {
+        case 21: return run_ntt3<F, INV, 21, false, 0, true>(ctx, f, pl, data, src, mul, batch, src_len, dst_len, mul_mask, nullptr, coset);
+        case 22: return run_ntt3<F, INV, 22, false, 0, true>(ctx, f, pl, data, src, mul, batch, src_len, dst_len, mul_mask, nullptr, coset);
+        case 23: return run_ntt3<F, INV, 23, false, 0, true>(ctx, f, pl, data, src, mul, batch, src_len, dst_len, mul_mask, nullptr, coset);
+        case 24: return run_ntt3<F, INV, 24, false, 0, true>(ctx, f, pl, data, src, mul, batch, src_len, dst_len, mul_mask, nullptr, coset);
+        default: break;
+      }
+    } else if (ctx->tune.ntt3 && !(INV && mul)) {   // mul_mask: one multiplier word per output (~0) or a shared n-word one (n - 1)
       const bool bounded = src_len != NTT_UNBOUNDED || dst_len != NTT_UNBOUNDED;  // only ever with batch == 1
       // 2^16: worth it once the grid fills the GPU (16 tiles per transform); single transforms stay launch-bound
       if (log_n == 24 && !bounded) return run_ntt3<F, INV, 24, false>(ctx, f, pl, data, src, mul, batch, src_len, dst_len, mul_mask);
@@ -459,18 +491,30 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
                                   log_n, batch, tile1, tile2, &tiles);
   A1.src_len = src_len;
   if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
+  if (coset) {   // the hooked pass is the first (forward) or the last (inverse); launch_tile_n picks it
+    A1.coset_lo = coset;
+    A1.coset_hi = coset + ((size_t)1 << coset_h);
+    A1.coset_h = coset_h;
+  }
   if (ctx->tune.tw_table) {
     const u64* tab = nullptr;
     RONK_TRY(interpass_table(ctx, f, pl, INV, A1.log_c2, A1.tw_lo, A1.tw_hi, &tab));
     A1.tw_full = tab;
   }
-  RONK_TRY((launch_tile<F, MODE_PASS1, INV>(ctx, f, A1, (u32)tiles, INV ? "intt_pass1" : "ntt_pass1")));
+  const char* name1 = coset ? (INV ? "intt_pass1_coset" : "ntt_pass1_coset") : (INV ? "intt_pass1" : "ntt_pass1");
+  RONK_TRY((launch_tile<F, MODE_PASS1, INV>(ctx, f, A1, (u32)tiles, name1)));
   // pass 2: N2-point transforms along the contiguous workspace tiles, natural-order output
   NttTileArgs A2 = ntt_args_pass2(ws, data, mul, pl.tw2_2d[INV ? 1 : 0], log_n, batch, tile2, &tiles);
   A2.dst_len = dst_len;
   A2.mul_mask = mul_mask;
   if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
-  return launch_tile<F, MODE_PASS2, INV>(ctx, f, A2, (u32)tiles, INV ? "intt_pass2" : "ntt_pass2");
+  if (coset) {
+    A2.coset_lo = coset;
+    A2.coset_hi = coset + ((size_t)1 << coset_h);
+    A2.coset_h = coset_h;
+  }
+  const char* name2 = coset ? (INV ? "intt_pass2_coset" : "ntt_pass2_coset") : (INV ? "intt_pass2" : "ntt_pass2");
+  return launch_tile<F, MODE_PASS2, INV>(ctx, f, A2, (u32)tiles, name2);
 }
 
 template <class F>
@@ -529,6 +573,27 @@ int ntt_single_tables(ronk_ctx* ctx, u64 p, u64 g, u32 log_n, const u64** fwd, c
     return RONK_OK;
   });
 }
+
+// A coset transform with s != 1 (ntt_coset.cu checks the arguments; log_n >= 1): the two coset tables in this call's
+// scratch, built by one launch, then run_ntt with the factor fused into its first or last pass.
+int ntt_device_coset(ronk_ctx* ctx, u64 p, u64 g, u64* data, u32 log_n, u32 batch, u64 shift, int inverse) {
+  return with_field(ctx, p, g, inverse != 0, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    NttPlan* pl = nullptr;
+    RONK_TRY(plan_for(ctx, f, p, g, log_n, &pl));
+    const u32 h = (log_n + 1) / 2;
+    const u32 words = (1u << h) + (1u << (log_n - h));
+    Frame fr(ctx);
+    u64* tab = nullptr;
+    RONK_TRY(fr.take(&tab, words));
+    const u64 c = inverse ? h_powmod(shift, p - 2, p) : shift;
+    RONK_TRY(launch(ctx, "ntt_coset_table", coset_table_kernel<F>, (words + 255) / 256, 256, 0, false, f, c, h, log_n, tab));
+    return inverse ? run_ntt<F, true>(ctx, f, *pl, data, nullptr, batch, nullptr, NTT_UNBOUNDED, NTT_UNBOUNDED, ~0ULL, tab)
+                   : run_ntt<F, false>(ctx, f, *pl, data, nullptr, batch, nullptr, NTT_UNBOUNDED, NTT_UNBOUNDED, ~0ULL, tab);
+  });
+}
+
+size_t ntt_workspace_words(u32 log_n, u32 batch) { return ntt_shape(log_n).two_pass ? (size_t)batch << log_n : 0; }
 
 int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n, u32 batch, int inverse) {
   if (!ctx || !data) return set_err(ctx, RONK_EINVAL, "null argument");

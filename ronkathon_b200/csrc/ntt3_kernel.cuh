@@ -104,7 +104,11 @@ struct Ntt3Args {
                        // every transform of the batch (the twiddle column of the distributed transform)
   u64 src_len;         // BOUNDED kernels (batch = 1): the first pass reads src[0, src_len) zero-extended,
   u64 dst_len;         //                               the last pass stores dst[0, dst_len) only
-  u64 scale_tw;        // ntt3p_kernel, inverse only: R^-1 in twiddle form (the sub-transforms' tables carry n'^-1, not n^-1)
+  union {
+    u64 scale_tw;        // ntt3p_kernel, inverse only: R^-1 in twiddle form (the sub-transforms' tables carry n'^-1, not n^-1)
+    const u64* coset;    // COSET passes (first pass forward, last pass inverse, 2^21 … 2^24): c^j = coset[j mod 2^h] ·
+                         // coset[2^h + (j >> h)], twiddle form, h = ⌈log2 n / 2⌉, j = index within the transform
+  };
   u32 batch;
   u32 flags;           // NTT_FLAG_MUL
 };
@@ -114,12 +118,14 @@ struct Ntt3Args {
 // PASS 3:    group g ↔ (col = g >> 4, d0 = g & 15): element q is i = 16 q + d0 of column col (i is the contiguous axis).
 // First pass of 2^21 … 2^23 (LR0 = log2 R0 < 4, PASS 1 only): register q = u·R0 + d1 is row 16·d1 + d0 of sub-transform u,
 // whose sixteen columns start 16·u after this thread's; radix_network<LR0> runs the 16 / R0 networks side by side.
+// COSET (first pass of 2^21 … 2^24 only): each word is multiplied by c^j, j its index within its transform (n = 2^(20 + LR0)).
 // Last pass of a SPLIT transform (n = 2^LI · n', LI > 0, PASS 3 only): the sixteen columns of the tile are 16 / 2^LI
 // consecutive k1' of EACH of the 2^LI sub-transforms (column c ↔ sub-transform c mod 2^LI, sub_stride = n' words apart),
 // so that the stores of round 1 — X[sub + 2^LI·k'] — are again sixteen contiguous words.
-template <class F, int PASS, bool INV, bool BOUNDED = false, int NG = 2, int LR0 = 4, int LI = 0>
+template <class F, int PASS, bool INV, bool BOUNDED = false, int NG = 2, int LR0 = 4, int LI = 0, bool COSET = false>
 RONK_DEV void n3_round0(const F& f, u64* smem, const Ntt3Args& A, u64 tile_base, u64 row_stride, u64 col_stride, u32 tid,
                         u64 sub_stride = 0) {
+  static_assert(!COSET || (PASS == 1 && !BOUNDED && LI == 0), "coset: the unbounded first pass of 2^21 … 2^24");
   constexpr u32 R0 = 1u << LR0;
 #if RONK_NTT3_UNROLL_GROUPS == 1
 #pragma unroll 1
@@ -150,6 +156,11 @@ RONK_DEV void n3_round0(const F& f, u64* smem, const Ntt3Args& A, u64 tile_base,
       } else {
         x[q] = p[off];
       }
+      if constexpr (COSET) {
+        constexpr u32 LOGN = 20 + LR0, H = (LOGN + 1) / 2;
+        const u32 j = (u32)(tile_base + (u64)d0 * row_stride + (u64)c * col_stride + off) & ((1u << LOGN) - 1u);
+        x[q] = coset_mul(f, x[q], A.coset, A.coset + (1u << H), H, j);
+      }
     }
     radix_network<LR0, INV>(f, x);
     // ω_R^(d0·k_lo) = ω_256^(d0·k_lo·16/R0), k_lo = bitrev_LR0(register index mod R0); nothing to do where k_lo = 0
@@ -168,8 +179,10 @@ RONK_DEV void n3_round0(const F& f, u64* smem, const Ntt3Args& A, u64 tile_base,
 // ---- round 1 + inter-pass twiddle + stores ----
 // group g ↔ (d1 = g >> 4, c = g & 15).  Register q is tile position d0 = q, i.e. output k = bitrev8(16 d1 + q) =
 // 16·bitrev4(q) + bitrev4(d1); it goes to row k of the output view, column c.
-template <class F, int PASS, bool INV, bool BOUNDED = false, int LOGN = 24, int NG = 2>
+// COSET (last pass of 2^21 … 2^24 only): each output word is multiplied by c^j, j its index within its transform.
+template <class F, int PASS, bool INV, bool BOUNDED = false, int LOGN = 24, int NG = 2, bool COSET = false>
 RONK_DEV void n3_round1(const F& f, const u64* smem, const Ntt3Args& A, u64 tile_base, u64 row_stride, u32 m_base, u32 tid) {
+  static_assert(!COSET || (PASS == 3 && !BOUNDED && LOGN >= 21), "coset: the unbounded last pass of 2^21 … 2^24");
   constexpr u32 LO = (u32)(LOGN + 1) / 2u;                // two-level twiddle tables (the plan's split): ω_n^x, x < 2^LO, and ω_n^(2^LO·y)
   constexpr u32 EMASK = (1u << LOGN) - 1u;                // exponents mod n
   constexpr bool P1 = PASS == 1 && LOGN >= 21;            // first pass of 2^21 … 2^24: R = 16·R0 points, 16 / R0 column blocks per tile
@@ -283,6 +296,11 @@ RONK_DEV void n3_round1(const F& f, const u64* smem, const Ntt3Args& A, u64 tile
 #pragma unroll
         for (int qp = 0; qp < 16; qp++)
           if (!BOUNDED || idx0 + (u64)qp * 16u * row_stride < A.dst_len) o[(u64)qp * 16u * row_stride] = f.mul(x[n3_br4(qp)], w[qp]);
+      } else if constexpr (COSET) {
+#pragma unroll
+        for (int qp = 0; qp < 16; qp++)
+          o[(u64)qp * 16u * row_stride] =
+              coset_mul(f, x[n3_br4(qp)], A.coset, A.coset + (1u << LO), LO, (u32)(idx0 + (u64)qp * 16u * row_stride) & EMASK);
       } else {
 #pragma unroll
         for (int qp = 0; qp < 16; qp++)
@@ -473,7 +491,8 @@ RONK_DEV void n3c_point(const F& f, const Ntt3Args& A, u64 b, u64 k2) {
 }
 
 #if defined(__CUDACC__)
-template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int NG = 2, int LI = 0>
+// COSET: the coset factor of Ntt3Args::coset_lo on the loads of PASS 1 (forward) or the stores of PASS 3 (inverse), 2^21 … 2^24.
+template <class F, int PASS, bool INV, int LOGN, bool BOUNDED, int NG = 2, int LI = 0, bool COSET = false>
 __global__ void __launch_bounds__(N3_THREADS * (2 / NG), RONK_NTT3_MINB / (2 / NG)) ntt3_kernel(const F f, const Ntt3Args A) {
   __shared__ u64 smem[N3_TILE_WORDS];
   const u32 tid = threadIdx.x;
@@ -484,10 +503,10 @@ __global__ void __launch_bounds__(N3_THREADS * (2 / NG), RONK_NTT3_MINB / (2 / N
   // not touch the predecessor's output before griddepcontrol.wait (no-ops without the launch attribute)
   asm volatile("griddepcontrol.launch_dependents;");
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  n3_round0<F, PASS, INV, BOUNDED && PASS == (LOGN >= 21 ? 1 : 2), NG, (PASS == 1 && LOGN >= 21) ? n3_log_r0(LOGN) : 4, LI>(
-      f, smem, A, in_base, in_row, in_col, tid, (u64)1 << LOGN);  // src_len: first pass only
+  n3_round0<F, PASS, INV, BOUNDED && PASS == (LOGN >= 21 ? 1 : 2), NG, (PASS == 1 && LOGN >= 21) ? n3_log_r0(LOGN) : 4, LI,
+            COSET && !INV>(f, smem, A, in_base, in_row, in_col, tid, (u64)1 << LOGN);  // src_len: first pass only
   __syncthreads();
-  n3_round1<F, PASS, INV, BOUNDED, LOGN, NG>(f, smem, A, out_base, out_row, m_base, tid);
+  n3_round1<F, PASS, INV, BOUNDED, LOGN, NG, COSET && INV>(f, smem, A, out_base, out_row, m_base, tid);
 }
 
 // One 2^16-point transform per 16-CTA cluster, in place (see the header comment).  256 threads, one group each.

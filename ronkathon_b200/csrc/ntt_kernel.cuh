@@ -58,7 +58,19 @@ struct NttTileArgs {
   u32 log_n, log_n1, log_n2, log_c2, log_lo;
   u32 tiles_per_batch;
   u32 flags;
+  // Coset transforms (COSET instantiations): the word at natural index j of each transform (global index mod n) is
+  // multiplied by c^j = coset_lo[j mod 2^coset_h] · coset_hi[j >> coset_h] (twiddle form), in the load of the first pass
+  // (forward, c = s) or the store of the last pass (inverse, c = s^-1, after the n^-1 of the inverse).
+  const u64* coset_lo;
+  const u64* coset_hi;
+  u32 coset_h;
 };
+
+// v · c^j from the two coset tables (see NttTileArgs::coset_lo): two general multiplies, no n-word table.
+template <class F>
+RONK_DEV u64 coset_mul(const F& f, u64 v, const u64* lo, const u64* hi, u32 h, u32 j) {
+  return f.mul_tw(v, f.mul_tw(lo[j & ((1u << h) - 1u)], hi[j >> h]));
+}
 
 // Shared-memory swizzle: 64-bit accesses are served per half-warp against 16 eight-byte banks
 // (low 4 bits of the element index).  XOR-folding bits [4,8), [8,12) and [12,14) into the bank
@@ -234,9 +246,11 @@ RONK_DEV void ntt_prefetch_pass1(const NttTileArgs& A, u32 tile, u32 tid, u32 nt
 #endif
 }
 
-// LD_BATCH loads into registers, then LD_BATCH swizzled stores (see above); BOUNDED adds `index < src_len`.
-template <int MODE, bool BOUNDED>
-RONK_DEV void ntt_load_batches(u64* smem, const NttTileArgs& A, u64 gaddr_t, u32 sw_t, u32 kk, u32 per_thread) {
+// LD_BATCH loads into registers, then LD_BATCH swizzled stores (see above); BOUNDED adds `index < src_len`; COSET
+// multiplies each word by c^j on its way to shared memory (f is used only then).
+template <int MODE, bool BOUNDED, bool COSET = false, class F = GoldilocksField>
+RONK_DEV void ntt_load_batches(u64* smem, const NttTileArgs& A, u64 gaddr_t, u32 sw_t, u32 kk, u32 per_thread,
+                               const F* f = nullptr) {
   for (u32 j0 = 0; j0 < per_thread; j0 += LD_BATCH) {
     u64 v[LD_BATCH];
 #pragma unroll
@@ -250,6 +264,7 @@ RONK_DEV void ntt_load_batches(u64* smem, const NttTileArgs& A, u64 gaddr_t, u32
         if (MODE == MODE_SINGLE) ok = g < A.total;
         if (BOUNDED) ok = ok && g < A.src_len;
         v[i] = ok ? A.src[g] : 0ULL;
+        if constexpr (COSET) v[i] = coset_mul(*f, v[i], A.coset_lo, A.coset_hi, A.coset_h, (u32)g & ((1u << A.log_n) - 1u));
       }
     }
 #pragma unroll
@@ -260,8 +275,8 @@ RONK_DEV void ntt_load_batches(u64* smem, const NttTileArgs& A, u64 gaddr_t, u32
   }
 }
 
-template <class F, int MODE, bool BOUNDED = false>
-RONK_DEV void ntt_load_phase(u64* smem, const NttTileArgs& A, u32 tile, u32 tid, u32 nthr) {
+template <class F, int MODE, bool BOUNDED = false, bool COSET = false>
+RONK_DEV void ntt_load_phase(u64* smem, const NttTileArgs& A, u32 tile, u32 tid, u32 nthr, const F* f = nullptr) {
   const u32 T = 1u << A.tile_log;
   const u32 kk = ilog2(nthr);
   u32 b = 0, sub = tile;
@@ -277,7 +292,7 @@ RONK_DEV void ntt_load_phase(u64* smem, const NttTileArgs& A, u32 tile, u32 tid,
   else gaddr_t = ((u64)b << A.log_n) + ((u64)sub << A.tile_log) + tid;
   const u32 sw_t = swz(tid);
   const u32 per_thread = T >> kk;  // elements per thread (T ≥ nthr)
-  ntt_load_batches<MODE, BOUNDED>(smem, A, gaddr_t, sw_t, kk, per_thread);
+  ntt_load_batches<MODE, BOUNDED, COSET>(smem, A, gaddr_t, sw_t, kk, per_thread, f);
 }
 
 // Round schedule: full radix-16 rounds from the top of the NTT index down, then one partial
@@ -435,8 +450,8 @@ RONK_DEV void ntt_store_phase(const F& f, const u64* smem, const NttTileArgs& A,
 }
 
 // ---- previous formulation of the phases (index math per element), kept selectable per mode ----
-template <class F, int MODE, bool BOUNDED = false>
-RONK_DEV void ntt_load_phase_v0(u64* smem, const NttTileArgs& A, u32 tile, u32 tid, u32 nthr) {
+template <class F, int MODE, bool BOUNDED = false, bool COSET = false>
+RONK_DEV void ntt_load_phase_v0(u64* smem, const NttTileArgs& A, u32 tile, u32 tid, u32 nthr, const F* f = nullptr) {
   const u32 T = 1u << A.tile_log;
   u32 b = 0, sub = tile;
   if (MODE != MODE_SINGLE) {
@@ -468,7 +483,13 @@ RONK_DEV void ntt_load_phase_v0(u64* smem, const NttTileArgs& A, u32 tile, u32 t
 #pragma unroll
     for (int i = 0; i < LB; i++) {
       const u32 e = e0 + i * nthr;
-      if (e < T) smem[swz(e)] = v[i];
+      if constexpr (COSET) {   // the factor once the whole batch of loads is in flight: a word's registers die at its store
+        static_assert(MODE != MODE_PASS2, "coset: the first pass");
+        const u64 g = MODE == MODE_SINGLE ? base + e : base + ((u64)(e >> A.log_c) << A.log_n2) + (e & cmask);
+        if (e < T) smem[swz(e)] = coset_mul(*f, v[i], A.coset_lo, A.coset_hi, A.coset_h, (u32)g & ((1u << A.log_n) - 1u));
+      } else {
+        if (e < T) smem[swz(e)] = v[i];
+      }
     }
   }
 }
@@ -476,7 +497,7 @@ RONK_DEV void ntt_load_phase_v0(u64* smem, const NttTileArgs& A, u32 tile, u32 t
 // FMUL (pass 2 only): the caller guarantees NTT_FLAG_MUL; the point-wise operand is then fetched in batches
 // ahead of the stores — in the plain loop every mul_src load sits behind the previous store (the two arrays
 // may alias as far as the compiler knows) and pays a full memory latency per element.
-template <class F, int MODE, bool INV, bool BOUNDED = false, bool FMUL = false>
+template <class F, int MODE, bool INV, bool BOUNDED = false, bool FMUL = false, bool COSET = false>
 RONK_DEV void ntt_store_phase_v0(const F& f, const u64* smem, const NttTileArgs& A, u32 tile, u32 tid, u32 nthr) {
   const u32 T = 1u << A.tile_log;
   const u32 M = 1u << A.log_m;
@@ -493,6 +514,7 @@ RONK_DEV void ntt_store_phase_v0(const F& f, const u64* smem, const NttTileArgs&
       const u32 e = (bt << A.log_m) | bitrev(k, A.log_m);
       u64 v = smem[swz(e)];
       if (A.flags & NTT_FLAG_SCALE) v = f.mul_tw(v, A.scale);
+      if constexpr (COSET) v = coset_mul(f, v, A.coset_lo, A.coset_hi, A.coset_h, (u32)(base + g) & (M - 1u));
       if (A.flags & NTT_FLAG_MUL) v = f.mul(v, A.mul_src[(base + g) & A.mul_mask]);
       A.dst[base + g] = v;
     }
@@ -545,6 +567,7 @@ RONK_DEV void ntt_store_phase_v0(const F& f, const u64* smem, const NttTileArgs&
         const u64 addr = base + k1_in + ((u64)k2 << A.log_n1);
         if (BOUNDED && addr >= A.dst_len) continue;
         u64 v = smem[swz(e)];
+        if constexpr (COSET) v = coset_mul(f, v, A.coset_lo, A.coset_hi, A.coset_h, (u32)addr & ((1u << A.log_n) - 1u));
         if (A.flags & NTT_FLAG_MUL) v = f.mul(v, A.mul_src[addr & A.mul_mask]);
         A.dst[addr] = v;
       }
@@ -681,8 +704,13 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, u
 
 // Shared memory: [ tile: T·8 B | twiddles: M·8 B | mbarrier: 8 B ]
 // BOUNDED instantiations (poly_mul only) honour A.src_len / A.dst_len; the unbounded ones carry no such code.
-template <class F, int MODE, bool INV, int NTHR, int MINB, bool BOUNDED = false, bool FMUL = false>
+// COSET instantiations (unbounded, no point-wise product) apply the coset factor c^j of NttTileArgs::coset_lo: forward in
+// the load of MODE_SINGLE / MODE_PASS1, inverse in the store of MODE_SINGLE / MODE_PASS2.
+template <class F, int MODE, bool INV, int NTHR, int MINB, bool BOUNDED = false, bool FMUL = false, bool COSET = false>
 __global__ void __launch_bounds__(NTHR, MINB) ntt_tile_kernel(const F f, const NttTileArgs A) {
+  static_assert(!COSET || (!BOUNDED && !FMUL && (MODE == MODE_SINGLE || (MODE == MODE_PASS1) != INV)),
+                "coset: unbounded, forward first pass or inverse last pass");
+  static_assert(!COSET || !INV || ((RONK_STORE_V0_MASK >> MODE) & 1), "the inverse coset factor is in the per-element store");
   extern __shared__ __align__(128) u64 smem[];
   const u32 tid = threadIdx.x, tile = blockIdx.x;
   const u32 T = 1u << A.tile_log;
@@ -700,8 +728,13 @@ __global__ void __launch_bounds__(NTHR, MINB) ntt_tile_kernel(const F f, const N
   // visible.  Both instructions are no-ops when the launch carries no PDL attribute.
   if (MODE == MODE_PASS1) asm volatile("griddepcontrol.launch_dependents;");
   if (MODE == MODE_PASS2) asm volatile("griddepcontrol.wait;" ::: "memory");
-  if ((RONK_LOAD_V0_MASK >> MODE) & 1) ntt_load_phase_v0<F, MODE, BOUNDED>(smem, A, tile, tid, NTHR);
-  else ntt_load_phase<F, MODE, BOUNDED>(smem, A, tile, tid, NTHR);
+  if constexpr (COSET && !INV) {
+    if ((RONK_LOAD_V0_MASK >> MODE) & 1) ntt_load_phase_v0<F, MODE, false, true>(smem, A, tile, tid, NTHR, &f);
+    else ntt_load_phase<F, MODE, false, true>(smem, A, tile, tid, NTHR, &f);
+  } else {
+    if ((RONK_LOAD_V0_MASK >> MODE) & 1) ntt_load_phase_v0<F, MODE, BOUNDED>(smem, A, tile, tid, NTHR);
+    else ntt_load_phase<F, MODE, BOUNDED>(smem, A, tile, tid, NTHR);
+  }
   if (MODE == MODE_PASS1 && A.prefetch_dist && tile + A.prefetch_dist < gridDim.x)
     ntt_prefetch_pass1(A, tile + A.prefetch_dist, tid, NTHR);
   __syncthreads();
@@ -711,7 +744,7 @@ __global__ void __launch_bounds__(NTHR, MINB) ntt_tile_kernel(const F f, const N
     ntt_round_dispatch<F, INV>(f, smem, tw, A, nst, wb, lcur, tid, NTHR);
     __syncthreads();
   }
-  if ((RONK_STORE_V0_MASK >> MODE) & 1) ntt_store_phase_v0<F, MODE, INV, BOUNDED, FMUL>(f, smem, A, tile, tid, NTHR);
+  if ((RONK_STORE_V0_MASK >> MODE) & 1) ntt_store_phase_v0<F, MODE, INV, BOUNDED, FMUL, COSET && INV>(f, smem, A, tile, tid, NTHR);
   else ntt_store_phase<F, MODE, INV, BOUNDED>(f, smem, A, tile, tid, NTHR);
 }
 
@@ -747,6 +780,14 @@ template <class F>
 __global__ void pow_table_kernel(const F f, u64 w, u64 s, u64* tab, u32 count) {
   const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < count) tab[i] = f.to_tw(f.mul(field_pow(f, w, (u64)i), s));
+}
+// The two coset tables of a coset transform of 2^log_n points, h = ⌈log_n / 2⌉ (c plain):
+// out[i] = to_tw(c^i) for i < 2^h, out[2^h + i] = to_tw(c^(i·2^h)) for i < 2^(log_n - h).
+template <class F>
+__global__ void coset_table_kernel(const F f, u64 c, u32 h, u32 log_n, u64* out) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x, lo = 1u << h;
+  if (i >= lo + (1u << (log_n - h))) return;
+  out[i] = f.to_tw(field_pow(f, c, i < lo ? (u64)i : (u64)(i - lo) << h));
 }
 #endif  // __CUDACC__
 

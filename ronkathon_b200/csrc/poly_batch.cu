@@ -35,8 +35,6 @@ constexpr u32 kFusedMaxLog = PM_MAX_LOG;
 // words wherever the batched transforms run.
 constexpr u64 kBatchMaxWords = (u64)1 << 40, kBatchMaxTransformWords = (u64)1 << 32;
 
-constexpr int PAD_THREADS = 256;
-
 // dst[r·N + k] = k < d ? src[r·stride + k] : 0, over total = rows·N words.
 __global__ void __launch_bounds__(PAD_THREADS)
 poly_rows_pad_kernel(const u64* __restrict__ src, u32 d, u64 stride, u32 log_n, u64 total, u64* __restrict__ dst) {

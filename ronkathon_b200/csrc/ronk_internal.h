@@ -412,6 +412,12 @@ inline int with_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, Fn&& fn) {
 
 // Internal device-pointer entry points used across translation units.
 int ntt_device(ronk_ctx* ctx, u64 p, u64 g, u64* data, const u64* mul, u32 log_n, u32 batch, int inverse);
+// ntt.cu: batch in-place coset transforms on s·H_n, s != 1, log_n >= 1 (arguments checked by ntt_coset.cu): one launch
+// builds the factor tables in this call's scratch, then the transform runs with s^±j fused into its first or last pass.
+int ntt_device_coset(ronk_ctx* ctx, u64 p, u64 g, u64* data, u32 log_n, u32 batch, u64 shift, int inverse);
+// ntt.cu: the words of workspace a transform of batch × 2^log_n takes from the scratch on the single-tile and two-pass
+// kernels (and on the 256-point-tile passes that coset transforms take)
+size_t ntt_workspace_words(u32 log_n, u32 batch);
 int ntt_device_shared_mul(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64* dst, const u64* mul, u32 log_n, u32 batch);
 int ntt_device_bounded(ronk_ctx* ctx, u64 p, u64 g, const u64* src, u64 src_len, u64* dst, u64 dst_len, const u64* mul,
                        u32 log_n, int inverse);
@@ -462,6 +468,11 @@ size_t poly_mul_rows_pow2_scratch(const ronk_ctx* ctx, size_t da, size_t db, boo
 int crt_mul_rows_device(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, bool b_shared, u32 batch,
                         u64* c);
 size_t crt_mul_rows_scratch(const ronk_ctx* ctx, u64 p, size_t da, size_t db, bool b_shared, u32 batch);
+// poly_batch.cu: dst[r·N + k] = k < d ? src[r·stride + k] : 0 (N = 2^log_n) over total = rows·N words, a grid-stride
+// loop of PAD_THREADS-thread CTAs.  Zero-pads the rows of the batched product and of the LDE (ntt_coset.cu).
+constexpr int PAD_THREADS = 256;
+__global__ void __launch_bounds__(PAD_THREADS)
+poly_rows_pad_kernel(const u64* __restrict__ src, u32 d, u64 stride, u32 log_n, u64 total, u64* __restrict__ dst);
 // poly.cu: the schoolbook kernel over `batch` contiguous rows (b_stride = db, or 0 for one shared b).
 int poly_mul_schoolbook_rows(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, size_t b_stride,
                              u64 batch, u64* c);

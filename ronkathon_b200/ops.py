@@ -43,6 +43,28 @@ def ntt_any_(ctx: Context, data, n: int, batch: int = 1, inverse: bool = False, 
     return data
 
 
+def ntt_coset_(ctx: Context, data, log_n: int, shift: int, batch: int = 1, inverse: bool = False, p: int = GOLDILOCKS,
+               g: int = 7):
+    """In-place transforms on the coset shift·H_n over `batch` contiguous rows: forward X[k] = Σ_j a_j (shift·ω^k)^j,
+    inverse its inverse.  shift = 1 is ntt_."""
+    _check_u64(data)
+    assert data.numel() == (batch << log_n)
+    ctx.call("ronk_ntt_coset_u64", p, g, _lib._ptr(data), log_n, batch, shift, int(inverse))
+    return data
+
+
+def lde(ctx: Context, coeffs, log_n: int, shift: int, p: int = GOLDILOCKS, g: int = 7):
+    """Low-degree extension: the coefficients (d,) — or rows (batch, d) — evaluated on shift·H_N, N = 2^log_n ≥ d.
+    Returns a new (N,) — or (batch, N) — tensor."""
+    import torch
+    _check_u64(coeffs)
+    assert coeffs.dim() in (1, 2), "coeffs is (d,) or (batch, d)"
+    batch, d = (1, coeffs.shape[0]) if coeffs.dim() == 1 else coeffs.shape
+    out = torch.empty(coeffs.shape[:-1] + (1 << log_n,), dtype=torch.int64, device=coeffs.device)
+    ctx.call("ronk_poly_lde_u64", p, g, _lib._ptr(coeffs), d, log_n, shift, batch, _lib._ptr(out))
+    return out
+
+
 def ntt_mul_(ctx: Context, data, mul, log_n: int, batch: int = 1, p: int = GOLDILOCKS, g: int = 7):
     """data ← NTT(data) ⊙ mul, the point-wise product fused into the last stage."""
     _check_u64(data); _check_u64(mul)
