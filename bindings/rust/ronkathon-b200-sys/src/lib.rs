@@ -79,6 +79,12 @@ extern "C" {
   pub fn ronk_poly_eval_u64(ctx: *mut ronk_ctx, p: u64, coeffs: *const u64, d: usize, xs: *const u64, m: usize, out: *mut u64) -> c_int;
   pub fn ronk_poly_eval_u64_host(ctx: *mut ronk_ctx, p: u64, coeffs: *const u64, d: usize, xs: *const u64, m: usize, out: *mut u64) -> c_int;
   pub fn ronk_poly_lagrange_eval_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, n: usize, x: u64, out: *mut u64) -> c_int;
+  /// Lagrange-basis rows (batch × n) on the coset shift·H_n at m points, barycentric, O(n) per point; device pointers.
+  pub fn ronk_poly_lagrange_eval_u64(ctx: *mut ronk_ctx, p: u64, g: u64, evals: *const u64, n: u64, batch: u32, shift: u64, xs: *const u64, m: usize, out: *mut u64) -> c_int;
+  pub fn ronk_poly_lagrange_eval_batch_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, evals: *const u64, n: u64, batch: u32, shift: u64, xs: *const u64, m: usize, out: *mut u64) -> c_int;
+  /// `kzg::open` in evaluation form (src/kzg/setup.rs:63-78): f_b(z) and the quotient's evaluations on the nodes.
+  pub fn ronk_poly_lagrange_open_u64(ctx: *mut ronk_ctx, p: u64, g: u64, evals: *const u64, n: u64, batch: u32, shift: u64, z: u64, values: *mut u64, quotient: *mut u64) -> c_int;
+  pub fn ronk_poly_lagrange_open_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, evals: *const u64, n: u64, batch: u32, shift: u64, z: u64, values: *mut u64, quotient: *mut u64) -> c_int;
   pub fn ronk_poly_divrem_u64_host(ctx: *mut ronk_ctx, p: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;
   /// `quotient_and_remainder` on device pointers; Newton iteration on the transforms when the divisor's top word is nonzero.
   pub fn ronk_poly_divrem_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;

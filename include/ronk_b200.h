@@ -273,6 +273,41 @@ int ronk_poly_eval_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *coeffs, s
  * is a node, because l(x) = 0 multiplies the fold).  Host pointers, n | p-1.  RONK_EINVAL when two
  * nodes coincide (ω of order below n: the reference divides by zero). */
 int ronk_poly_lagrange_eval_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t n, uint64_t x, uint64_t *out);
+/* Lagrange-basis rows on a coset, evaluated at many points and opened at one point, in O(n) per point and row.
+ * Nodes x_j = s·ω^j, j < n, ω = g^((p-1)/n), s = `shift` (s = 1: the reference's nodes, mod.rs:363).  Any n | p - 1.
+ * `evals` is batch × n, row-major: row b holds f_b(x_j).  With Z(X) = X^n - s^n and the weights w_j = x_j / (n·s^n):
+ *   eval:  out[b·m + i] = L_b(xs[i]) = Z(xs[i]) · Σ_j w_j·evals[b·n + j] / (xs[i] - x_j)   (out is batch × m).
+ *          At a node the value is 0, the reference's l(x)·fold; with s = 1 every word is the one the single-point
+ *          ronk_poly_lagrange_eval_u64_host above gives.
+ *   open:  values[b] = f_b(z), the true value (evals[b·n + k] when z = x_k), and quotient (batch × n) the evaluations on
+ *          the nodes of (f_b - f_b(z)) / (X - z): q_j = (y_j - f(z)) / (x_j - z); at z = x_k, q_k = f_b'(x_k).  This is
+ *          kzg::open (src/kzg/setup.rs:63-78) in evaluation form.
+ * - Errors, in this order: RONK_EINVAL for a null pointer; the modulus's (RONK_EUNSUPPORTED for p = 2); RONK_EINVAL for
+ *   g == 0 or g >= p, n == 0 or n not dividing p - 1; RONK_EUNSUPPORTED for n or batch·n above 2^32 words; RONK_EINVAL
+ *   when ω has order below n (two nodes coincide: the reference divides by zero, for every x), for shift == 0 or
+ *   shift >= p, and (open) z >= p; RONK_EUNSUPPORTED (eval) for batch·m above 2^32 words; RONK_EINVAL for an output that
+ *   overlaps an input, or values that overlap quotient.  Past those, RONK_EUNSUPPORTED (eval) for more than 2^31 - 1
+ *   tiles of nodes and points (about m·n > 2^42).  batch == 0 or m == 0 does nothing.
+ * - xs are taken as canonical and not read on the host; the _host twin refuses a non-canonical point (RONK_EINVAL) before
+ *   it stages anything.  Every check is made and all scratch is taken before the first launch; nothing is written on
+ *   failure.  Scratch: ω^-1's two power tables (2^h + 2^(⌈log2 n⌉ - h) words, h = ⌈⌈log2 n⌉ / 2⌉) and the per-CTA partial
+ *   sums, ⌈m / M⌉·⌈n·M / 4096⌉·batch·M words with M = 1, 2, 4 or 8 points per pass (at most 8, the smallest that holds m).
+ * - Kernels: one CTA forms its 4096 coefficients x_j / (x - x_j) with one batch inversion per 16 per thread, then streams
+ *   every row's tile through per-(row, point) accumulators, so each evaluation word is read once per group of 8 points;
+ *   a finish launch sums the partials in a fixed order and scales by Z(x) / (n·s^n).  The launch sequence depends only on
+ *   (p, g, n, shift), and for open on whether z ∈ s·H_n, which the host decides by (z/s)^n = 1:
+ *   off the nodes the evaluation at z, then one quotient launch; on a node the device finds k, the quotient launch gathers
+ *   the values, and the evaluation's partial and finish kernels fill q_k = -x_k^-1 Σ_{j≠k} x_j q_j.  Asynchronous on the
+ *   context's stream; no readback.  The _host twins stage in and out and synchronise (the batched evaluation's twin has
+ *   its own name, because the single-point Lagrange evaluate above holds the plain one). */
+int ronk_poly_lagrange_eval_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *evals, uint64_t n, uint32_t batch,
+                                uint64_t shift, const uint64_t *xs, size_t m, uint64_t *out);
+int ronk_poly_lagrange_eval_batch_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *evals, uint64_t n,
+                                           uint32_t batch, uint64_t shift, const uint64_t *xs, size_t m, uint64_t *out);
+int ronk_poly_lagrange_open_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *evals, uint64_t n, uint32_t batch,
+                                uint64_t shift, uint64_t z, uint64_t *values, uint64_t *quotient);
+int ronk_poly_lagrange_open_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *evals, uint64_t n, uint32_t batch,
+                                     uint64_t shift, uint64_t z, uint64_t *values, uint64_t *quotient);
 /* quotient_and_remainder / Div / Rem — src/polynomial/mod.rs:170-225, arithmetic.rs:121-146.
  * q and r both have da terms.  Host pointers: ronk_poly_divrem_u64 below with g = 0, so a divisor that is not linear
  * keeps the literal long division.  RONK_EINVAL for an all-zero divisor. */

@@ -138,6 +138,29 @@ struct Polynomial {
     }
     return out;
   }
+  // evaluate at many points (Lagrange: the barycentric form in O(n) per point, 0 at a node, as evaluate)
+  std::vector<F> evaluate_many(const std::vector<F>& xs) const {
+    auto raw = to_raw();
+    std::vector<uint64_t> rx(xs.size()), out(xs.size());
+    for (size_t i = 0; i < xs.size(); i++) rx[i] = xs[i].value;
+    if constexpr (std::is_same_v<B, Monomial>) {
+      ctx().check(ronk_poly_eval_u64_host(ctx().get(), F::ORDER, raw.data(), raw.size(), rx.data(), rx.size(), out.data()));
+    } else {
+      ctx().check(ronk_poly_lagrange_eval_batch_u64_host(ctx().get(), F::ORDER, F::PRIMITIVE_ELEMENT().value, raw.data(),
+                                                         raw.size(), 1, 1, rx.data(), rx.size(), out.data()));
+    }
+    return from_raw(out);
+  }
+  // kzg::open (kzg/setup.rs:63-78) in evaluation form: f(z) and the evaluations of (f - f(z)) / (X - z) on the nodes
+  std::pair<F, Polynomial> open(F z) const {
+    static_assert(std::is_same_v<B, Lagrange>);
+    auto raw = to_raw();
+    std::vector<uint64_t> q(raw.size());
+    F v;
+    ctx().check(ronk_poly_lagrange_open_u64_host(ctx().get(), F::ORDER, F::PRIMITIVE_ELEMENT().value, raw.data(), raw.size(),
+                                                 1, 1, z.value, &v.value, q.data()));
+    return {v, Polynomial(from_raw(q))};
+  }
   size_t degree() const {  // polynomial/mod.rs:113-115
     for (size_t i = coefficients.size(); i-- > 0;)
       if (coefficients[i] != F::ZERO()) return i;

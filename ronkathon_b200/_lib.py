@@ -72,6 +72,10 @@ SIGNATURES = {
     "ronk_poly_eval_u64": (i32, [vp, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_eval_u64_host": (i32, [vp, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_lagrange_eval_u64_host": (i32, [vp, u64, u64, vp, sz, u64, p64]),
+    "ronk_poly_lagrange_eval_u64": (i32, [vp, u64, u64, vp, u64, u32, u64, vp, sz, vp]),
+    "ronk_poly_lagrange_eval_batch_u64_host": (i32, [vp, u64, u64, vp, u64, u32, u64, vp, sz, vp]),
+    "ronk_poly_lagrange_open_u64": (i32, [vp, u64, u64, vp, u64, u32, u64, u64, vp, vp]),
+    "ronk_poly_lagrange_open_u64_host": (i32, [vp, u64, u64, vp, u64, u32, u64, u64, vp, vp]),
     "ronk_poly_divrem_u64_host": (i32, [vp, u64, vp, sz, vp, sz, vp, vp]),
     "ronk_poly_divrem_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp, vp]),
     "ronk_poly_div_linear_u64": (i32, [vp, u64, vp, sz, u64, u64, vp, vp]),

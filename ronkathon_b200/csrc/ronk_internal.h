@@ -393,6 +393,20 @@ inline u32 log2_ceil(u64 v) {
 // Whether the power-of-two transforms take 2^log_n points over p: log_n ≤ 26 and 2^log_n divides p - 1.
 inline bool pow2_fits(u64 p, u32 log_n) { return log_n <= 26 && (p - 1) % ((u64)1 << log_n) == 0; }
 
+// Whether w, given w^n = 1 mod p, has order exactly n: w^(n/q) != 1 for every prime q dividing n.  Trial division, so
+// under 2^16 steps for n ≤ 2^32.  Where it fails, two of the points ω^i, i < n, coincide (Reed–Solomon positions,
+// barycentric nodes) and the reference divides by zero.
+inline bool root_has_order(u64 w, u64 n, u64 p) {
+  u64 r = n;
+  for (u64 q = 2; r > 1; q++) {
+    if (q * q > r) q = r;
+    if (r % q) continue;
+    if (h_powmod(w, n / q, p) == 1) return false;
+    while (r % q == 0) r /= q;
+  }
+  return true;
+}
+
 int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out);  // ntt.cu
 int validate_modulus(ronk_ctx* ctx, u64 p);                                       // field_ops.cu
 

@@ -255,14 +255,8 @@ static bool bytes_overlap(const void* a, size_t na, const void* b, size_t nb) {
 static int rs_args(ronk_ctx* ctx, u64 p, u64 g, const void* in, u64 n, u64 k, u64 rows, AnyNttPath* path) {
   if (n == 0 || k == 0 || k > n) return set_err(ctx, RONK_EINVAL, "need 0 < k <= n");
   RONK_TRY(anyntt_args(ctx, p, g, in, n, path));
-  const u64 w = h_powmod(g, (p - 1) / n, p);
-  u64 r = n;  // n ≤ 2^26 here: each prime factor q of n must leave ω^(n/q) ≠ 1
-  for (u64 q = 2; r > 1; q++) {
-    if (q * q > r) q = r;
-    if (r % q) continue;
-    if (h_powmod(w, n / q, p) == 1) return set_err(ctx, RONK_EINVAL, "ω_n has order below n (two positions share a point)");
-    while (r % q == 0) r /= q;
-  }
+  if (!root_has_order(h_powmod(g, (p - 1) / n, p), n, p))  // n ≤ 2^26 here
+    return set_err(ctx, RONK_EINVAL, "ω_n has order below n (two positions share a point)");
   if (rows * n > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
   return RONK_OK;
 }

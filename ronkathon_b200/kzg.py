@@ -61,6 +61,23 @@ def commit_lagrange(evaluations, g1_srs) -> AffinePoint:
     return commit([int(v) for v in mono.coefficients], g1_srs)
 
 
+def open_lagrange(evaluations, eval_point, g1_srs) -> AffinePoint:
+    """kzg/setup.rs:63-78 in evaluation form: the polynomial given by its values on the n-th roots of unity of F17, opened
+    at z.  The quotient (f - f(z)) / (X - z) is formed on the same nodes in one O(n) pass (ronk_poly_lagrange_open_u64,
+    also where z is a node), then committed with commit_lagrange.  The same point as open_ on the monomial coefficients."""
+    from .polynomial import Lagrange
+    poly = evaluations if isinstance(evaluations, Polynomial) else Polynomial(evaluations, PlutoScalarField, Lagrange)
+    if poly.basis is not Lagrange:
+        raise _lib.RonkPanic(1, "open_lagrange expects a Lagrange-basis polynomial")
+    z = PlutoScalarField(getattr(eval_point, "value", eval_point))
+    n = len(poly.coefficients)
+    value = np.empty(1, dtype=np.uint64)
+    quotient = np.empty(n, dtype=np.uint64)
+    _lib.default_context().call("ronk_poly_lagrange_open_u64_host", poly.p, poly.g, _lib._ptr(poly.coefficients), n, 1, 1,
+                                z.value, _lib._ptr(value), _lib._ptr(quotient))
+    return commit_lagrange(Polynomial(quotient, PlutoScalarField, Lagrange), g1_srs)
+
+
 def commit_preprocessed(polys: dict, g1_srs) -> dict:
     """Commitments to a `CommonPreprocessedInput` (compiler/program.rs:59-63: ql, qr, qm, qo, qc, s1, s2, s3),
     each given as GROUP_ORDER evaluations."""

@@ -115,6 +115,39 @@ def poly_eval(ctx: Context, coeffs, xs, p: int = GOLDILOCKS):
     return out
 
 
+def _rows(evals, n: int):
+    """(n,) or (batch, n) evaluations → (batch, leading shape)."""
+    _check_u64(evals)
+    assert evals.dim() in (1, 2) and evals.shape[-1] == n, "evals is (n,) or (batch, n)"
+    return (1 if evals.dim() == 1 else evals.shape[0]), tuple(evals.shape[:-1])
+
+
+def lagrange_eval(ctx: Context, evals, xs, n: int, shift: int = 1, p: int = GOLDILOCKS, g: int = 7):
+    """Lagrange-basis rows on the coset shift·H_n (evals (n,) or (batch, n), row b holding f_b(shift·ω^j)) evaluated at
+    the m points xs, by the barycentric formula in O(n) per point: a new (m,) or (batch, m) tensor.  At a node the value
+    is 0, as the reference's Lagrange evaluate gives.  Asynchronous."""
+    import torch
+    batch, lead = _rows(evals, n)
+    _check_u64(xs)
+    out = torch.empty(lead + (xs.numel(),), dtype=torch.int64, device=evals.device)
+    ctx.call("ronk_poly_lagrange_eval_u64", p, g, _lib._ptr(evals), n, batch, shift, _lib._ptr(xs), xs.numel(),
+             _lib._ptr(out))
+    return out
+
+
+def lagrange_open(ctx: Context, evals, z: int, n: int, shift: int = 1, p: int = GOLDILOCKS, g: int = 7):
+    """Opens Lagrange-basis rows on shift·H_n at z: returns new tensors (values, quotient), values[b] = f_b(z) ((,) or
+    (batch,)) and quotient the evaluations of (f_b - f_b(z)) / (X - z) on the same nodes (the shape of evals).
+    Asynchronous."""
+    import torch
+    batch, lead = _rows(evals, n)
+    values = torch.empty(lead if lead else (1,), dtype=torch.int64, device=evals.device)
+    quotient = torch.empty_like(evals)
+    ctx.call("ronk_poly_lagrange_open_u64", p, g, _lib._ptr(evals), n, batch, shift, z, _lib._ptr(values),
+             _lib._ptr(quotient))
+    return (values if lead else values[0]), quotient
+
+
 def poly_from_roots(ctx: Context, xs, p: int = GOLDILOCKS, g: int = 7):
     """Π (X - xs[i]) — returns a new tensor of len(xs) + 1 coefficients (subproduct tree above the crossover)."""
     import torch

@@ -86,12 +86,16 @@ class Polynomial:
         return self.field(res.value)
 
     def evaluate_many(self, xs):
-        """Batched `evaluate` (one kernel, one CTA per point)."""
-        assert self.basis is Monomial
+        """Batched `evaluate`: one kernel with one CTA per point in the monomial basis; in the Lagrange basis the
+        barycentric form on the nodes ω^i, O(n) per point (0 at a node, as `evaluate`)."""
         xs = _coeffs(self.field, xs)
         out = np.empty(len(xs), dtype=np.uint64)
-        self._ctx().call("ronk_poly_eval_u64_host", self.p, _lib._ptr(self.coefficients), len(self.coefficients),
-                         _lib._ptr(xs), len(xs), _lib._ptr(out))
+        if self.basis is Monomial:
+            self._ctx().call("ronk_poly_eval_u64_host", self.p, _lib._ptr(self.coefficients), len(self.coefficients),
+                             _lib._ptr(xs), len(xs), _lib._ptr(out))
+        else:
+            self._ctx().call("ronk_poly_lagrange_eval_batch_u64_host", self.p, self.g, _lib._ptr(self.coefficients),
+                             len(self.coefficients), 1, 1, _lib._ptr(xs), len(xs), _lib._ptr(out))
         return [self.field(int(v)) for v in out]
 
     def pow_mult(self, d2: int, coeff):  # polynomial/mod.rs:153-157
