@@ -96,6 +96,14 @@ extern "C" {
   pub fn ronk_poly_multieval_u64(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, d: usize, xs: *const u64, m: usize, out: *mut u64) -> c_int;
   /// Device twin of `ronk_poly_interpolate_u64_host`; synchronous.
   pub fn ronk_poly_interpolate_u64(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, ys: *const u64, k: usize, out: *mut u64) -> c_int;
+  /// `evaluate` of `batch` rows (batch × d) at the same m points (Shamir split of many secrets), one shared tree; device
+  /// pointers, out batch × m; asynchronous.  Every row is the words of `ronk_poly_multieval_u64`.
+  pub fn ronk_poly_multieval_batch_u64(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, d: usize, batch: u32, xs: *const u64, m: usize, out: *mut u64) -> c_int;
+  pub fn ronk_poly_multieval_batch_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, coeffs: *const u64, d: usize, batch: u32, xs: *const u64, m: usize, out: *mut u64) -> c_int;
+  /// Interpolation of `batch` rows of ys (batch × k) through the same k nodes, one shared tree; device pointers, out
+  /// batch × k; synchronous.  Every row is the words of `ronk_poly_interpolate_u64`.
+  pub fn ronk_poly_interpolate_batch_u64(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, ys: *const u64, k: usize, batch: u32, out: *mut u64) -> c_int;
+  pub fn ronk_poly_interpolate_batch_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, ys: *const u64, k: usize, batch: u32, out: *mut u64) -> c_int;
   /// Division by b0 + b1·x (the divisor `kzg::open` builds, src/kzg/setup.rs:72-75) as a device-wide scan; device pointers.
   pub fn ronk_poly_div_linear_u64(ctx: *mut ronk_ctx, p: u64, a: *const u64, d: usize, b0: u64, b1: u64, q: *mut u64, rem: *mut u64) -> c_int;
 

@@ -352,6 +352,42 @@ int ronk_poly_multieval_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_
  * capped at 8192 nodes (RONK_EUNSUPPORTED above); the tree takes every k > 8192 it fits.  Synchronous; RONK_EINVAL for a
  * repeated x (the reference's `/` panics on the zero denominator). */
 int ronk_poly_interpolate_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *ys, size_t k, uint64_t *out);
+/* Batches over one shared point set (Shamir split and combine over many secrets, Message::decode of many codewords, a
+ * prover's columns at the same points): one tree per call, shared by every row.  DEVICE pointers, row-major.
+ * multieval: coeffs is batch × d, out is batch × m, out[b·m + i] = Σ_j coeffs[b·d + j]·xs[i]^j.
+ * interpolate: ys is batch × k, out is batch × k, row b the interpolant through (xs[i], ys[b·k + i]).
+ * - Words: every row is word for word what ronk_poly_multieval_u64 / ronk_poly_interpolate_u64 give for it.
+ * - Path rule: the tree runs where tree_fits, as for one row, and from a crossover that depends on the batch, because
+ *   the literal kernels' cost grows with it and the tree's barely does (DESIGN.md §5).  With n = min(d, m), multieval
+ *   takes the tree from n ≥ 2^15, batch·n² ≥ 2^30 or batch·n ≥ 2^18; interpolation from k ≥ 2048 or batch·k² ≥ 2^28,
+ *   and at every k > 8192.  At batch 1 that is the single-row rule.  RONK_TREE_MIN overrides it whatever the batch.
+ * - Launches: at batch 1 the launch sequence is the single-row entry's; from batch 2 it does not depend on the batch (save where ronk_ntt_u64 picks its
+ *   kernels by batch, at 2^16 points).  On the tree the node spectra are transformed once per level and met with every
+ *   row in one launch; interpolation evaluates M'(x_i) once and inverts it once.  Off the tree one poly_eval launch, or
+ *   one interp_master and one interp_nodes / interp_sum pair, serves every row.
+ * - Errors, in the single-row order: RONK_EINVAL for a null pointer, a bad modulus, g >= p; RONK_EUNSUPPORTED above 2^24
+ *   points; then RONK_EINVAL when out overlaps an input; RONK_EUNSUPPORTED when the tree's row buffers pass 2^32 words
+ *   (batch·N, N = 2^⌈log2 m⌉ or 2^⌈log2 k⌉, for multieval at least the root's 2^⌈log2(2d - 1)⌉, as
+ *   ronk_poly_mul_batch_u64), when off the tree the interpolation's partial sums pass 2^32 words
+ *   (batch·⌈k/256⌉·8·k), or for more than 8192 nodes off the tree.  interpolate: RONK_EINVAL for a repeated node (the
+ *   reference divides by zero), with out not written.  batch == 0, m == 0 or k == 0 does nothing.
+ * - Every check is made and all scratch is taken before the first launch; nothing is written on failure.  Scratch on
+ *   the tree: the stored levels (under 2N + 6·N/64 words), 2N words of node spectra, 3·batch·N words of rows (2N at
+ *   batch 1), for interpolation 2k words, the root's 2·N_q + d + 1 + min(m + 1, d) + 3·batch·d words (N_q =
+ *   2^⌈log2(2d - 1)⌉; interpolation evaluates M' as one row of k), and the largest transform workspace (batch·N words)
+ *   or batched product's.  Off the tree: none for multieval; batch·k + 2(k + 1) + batch·⌈k/256⌉·8·k words for
+ *   interpolation.
+ * - multieval is asynchronous.  interpolate synchronises once to read the repeated-node flag, as the single-row entry.
+ *   The _host twins make every check that reads no pointer, the size checks included, before they stage anything;
+ *   they stage in and out and synchronise. */
+int ronk_poly_multieval_batch_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t d, uint32_t batch,
+                                  const uint64_t *xs, size_t m, uint64_t *out);
+int ronk_poly_multieval_batch_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *coeffs, size_t d,
+                                       uint32_t batch, const uint64_t *xs, size_t m, uint64_t *out);
+int ronk_poly_interpolate_batch_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *ys, size_t k,
+                                    uint32_t batch, uint64_t *out);
+int ronk_poly_interpolate_batch_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *ys,
+                                         size_t k, uint32_t batch, uint64_t *out);
 int ronk_poly_div_linear_u64(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size_t d, uint64_t b0, uint64_t b1, uint64_t *q, uint64_t *rem);
 
 /* ---- Reed–Solomon codes ------------------------------------------------------------------- */

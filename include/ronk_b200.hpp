@@ -151,6 +151,24 @@ struct Polynomial {
     }
     return from_raw(out);
   }
+  // evaluate each of `polys` (monomial basis, equal lengths) at the same points (Shamir split of many secrets): one
+  // batched call sharing one subproduct tree; row b holds polys[b] at every xs[i]
+  static std::vector<std::vector<F>> evaluate_many_batch(const std::vector<Polynomial>& polys, const std::vector<F>& xs) {
+    static_assert(std::is_same_v<B, Monomial>);
+    const size_t d = polys.empty() ? 0 : polys[0].num_terms(), m = xs.size();
+    std::vector<uint64_t> rc(polys.size() * d), rx(m), out(polys.size() * m);
+    for (size_t b = 0; b < polys.size(); b++) {
+      if (polys[b].num_terms() != d) throw Panic("evaluate_many_batch: polynomials of different lengths");
+      for (size_t j = 0; j < d; j++) rc[b * d + j] = polys[b].coefficients[j].value;
+    }
+    for (size_t i = 0; i < m; i++) rx[i] = xs[i].value;
+    ctx().check(ronk_poly_multieval_batch_u64_host(ctx().get(), F::ORDER, F::PRIMITIVE_ELEMENT().value, rc.data(), d,
+                                                   (uint32_t)polys.size(), rx.data(), m, out.data()));
+    std::vector<std::vector<F>> rows(polys.size());
+    for (size_t b = 0; b < polys.size(); b++)
+      rows[b] = from_raw(std::vector<uint64_t>(out.begin() + b * m, out.begin() + (b + 1) * m));
+    return rows;
+  }
   // kzg::open (kzg/setup.rs:63-78) in evaluation form: f(z) and the evaluations of (f - f(z)) / (X - z) on the nodes
   std::pair<F, Polynomial> open(F z) const {
     static_assert(std::is_same_v<B, Lagrange>);
@@ -339,6 +357,24 @@ struct Message {  // reed_solomon.rs:13-17
     for (size_t i = 0; i < k; i++) { xs[i] = codeword[i].x.value; ys[i] = codeword[i].y.value; }
     Context::global().check(ronk_poly_interpolate_u64_host(Context::global().get(), F::ORDER, xs.data(), ys.data(), k, out.data()));
     return Message(Polynomial<Monomial, F>::from_raw(out));
+  }
+  // decode of many codewords whose first k coordinates share their x's: one batched interpolation over one tree
+  static std::vector<Message> decode_batch(const std::vector<std::vector<Coordinate<F>>>& codewords, size_t k) {
+    std::vector<uint64_t> xs(k), ys(codewords.size() * k), out(codewords.size() * k);
+    for (size_t b = 0; b < codewords.size(); b++) {
+      if (codewords[b].size() < k) throw Panic("Code size must be greater than or equal to K");
+      for (size_t i = 0; i < k; i++) {
+        if (b == 0) xs[i] = codewords[0][i].x.value;
+        else if (codewords[b][i].x.value != xs[i]) throw Panic("decode_batch: codewords on different x coordinates");
+        ys[b * k + i] = codewords[b][i].y.value;
+      }
+    }
+    Context::global().check(ronk_poly_interpolate_batch_u64_host(Context::global().get(), F::ORDER, F::PRIMITIVE_ELEMENT().value,
+                                                                 xs.data(), ys.data(), k, (uint32_t)codewords.size(), out.data()));
+    std::vector<Message> msgs;
+    for (size_t b = 0; b < codewords.size(); b++)
+      msgs.emplace_back(Polynomial<Monomial, F>::from_raw(std::vector<uint64_t>(out.begin() + b * k, out.begin() + (b + 1) * k)));
+    return msgs;
   }
 };
 

@@ -83,6 +83,10 @@ SIGNATURES = {
     "ronk_poly_from_roots_u64": (i32, [vp, u64, u64, vp, sz, vp]),
     "ronk_poly_multieval_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp]),
     "ronk_poly_interpolate_u64": (i32, [vp, u64, u64, vp, vp, sz, vp]),
+    "ronk_poly_multieval_batch_u64": (i32, [vp, u64, u64, vp, sz, u32, vp, sz, vp]),
+    "ronk_poly_multieval_batch_u64_host": (i32, [vp, u64, u64, vp, sz, u32, vp, sz, vp]),
+    "ronk_poly_interpolate_batch_u64": (i32, [vp, u64, u64, vp, vp, sz, u32, vp]),
+    "ronk_poly_interpolate_batch_u64_host": (i32, [vp, u64, u64, vp, vp, sz, u32, vp]),
     "ronk_rs_encode_u64": (i32, [vp, u64, u64, vp, u64, u64, u32, vp]),
     "ronk_rs_decode_u64": (i32, [vp, u64, u64, vp, vp, u64, u64, u32, vp, vp]),
     "ronk_rs_decode_u64_host": (i32, [vp, u64, u64, vp, vp, u64, u64, u32, vp, vp]),

@@ -8,8 +8,12 @@
 * Reed–Solomon errors-and-erasures correction (`rs_correct`): reads all N coordinates and corrects up to the
   decoding radius (`ronk_rs_decode_u64_host`).
 * Shamir `split` (src/shamir/mod.rs:53-58): `Polynomial::evaluate` at x = 1..n, one batched kernel.
+* Shamir `split_secret` / `combine_shares` over batches of secrets (`shamir_split`, `shamir_combine`): one batched
+  multipoint evaluation at x = 1..n, and one batched interpolation through the shares' x's.
 """
 from __future__ import annotations
+
+import secrets as _secrets
 
 import numpy as np
 
@@ -76,3 +80,46 @@ def shamir_shares(coefficients, n: int, field):
     """Evaluations of the sharing polynomial at x = 1..n (shamir/mod.rs:53-58), one kernel launch."""
     poly = Polynomial(coefficients, field)
     return list(zip(range(1, n + 1), poly.evaluate_many(range(1, n + 1))))
+
+
+def shamir_split(secrets, threshold: int, n: int, field, coefficients=None):
+    """split_secret (shamir/mod.rs:33-60) of every secret: returns (xs, ys) with xs = [1, …, n] and ys a (len(secrets), n)
+    array, row b the shares of secrets[b].  Row b's polynomial is secrets[b] + Σ_j coefficients[b][j-1]·X^j, j < threshold;
+    without `coefficients` they are drawn from the operating system's CSPRNG (`secrets.randbelow`).  One batched
+    multipoint evaluation on the device.  Panics (AssertionError) like the reference on threshold 0 or n < threshold."""
+    from . import _lib
+    assert threshold > 0, "threshold must be at least 1"
+    assert n >= threshold, "share count must be at least the threshold"
+    p = field.ORDER
+    assert n < p, "the share x's 1..n must be distinct field elements"
+    s = [int(getattr(v, "value", v)) % p for v in secrets]
+    if coefficients is None:
+        coefficients = [[_secrets.randbelow(p) for _ in range(threshold - 1)] for _ in s]
+    assert len(coefficients) == len(s) and all(len(c) == threshold - 1 for c in coefficients), \
+        "coefficients is len(secrets) rows of threshold - 1"
+    rows = np.array([[v] + [int(getattr(c, "value", c)) % p for c in cs] for v, cs in zip(s, coefficients)],
+                    dtype=np.uint64).reshape(len(s), threshold)
+    xs = np.arange(1, n + 1, dtype=np.uint64)
+    ys = np.empty((len(s), n), dtype=np.uint64)
+    if s:
+        _lib.default_context().call("ronk_poly_multieval_batch_u64_host", p, field.PRIMITIVE_ELEMENT.value,
+                                    _lib._ptr(rows), threshold, len(s), _lib._ptr(xs), n, _lib._ptr(ys))
+    return xs, ys
+
+
+def shamir_combine(shares_xs, shares_ys, field):
+    """combine_shares (shamir/mod.rs:76-97) of every row: shares_xs (k,) are the x's every secret's shares share,
+    shares_ys is (batch, k); returns the batch secrets as field elements.  The secret is coefficient 0 of the interpolant
+    through the shares, the reference's Lagrange sum at 0, also for more shares than the threshold.  One batched
+    interpolation on the device; a repeated x panics (RonkPanic) as the reference's inverse does."""
+    from . import _lib
+    p = field.ORDER
+    xs = np.array([int(getattr(x, "value", x)) % p for x in shares_xs], dtype=np.uint64)
+    k = len(xs)
+    assert k > 0, "at least one share is required"
+    ys = np.array([[int(getattr(y, "value", y)) % p for y in row] for row in shares_ys], dtype=np.uint64).reshape(-1, k)
+    out = np.empty_like(ys)
+    if len(ys):
+        _lib.default_context().call("ronk_poly_interpolate_batch_u64_host", p, field.PRIMITIVE_ELEMENT.value,
+                                    _lib._ptr(xs), _lib._ptr(ys), k, len(ys), _lib._ptr(out))
+    return [field(int(v)) for v in out[:, 0]]

@@ -36,27 +36,32 @@ __global__ void poly_mul_schoolbook_kernel(const F f, const u64* a, size_t da, c
   }
 }
 
-// evaluate (mod.rs:133-139): out[pt] = Σ_j c_j x^j.  One CTA per point; thread t owns the
-// coefficients j ≡ t (mod 256) (coalesced), Horner in x^256, then a shared-memory tree sum.
+// evaluate (mod.rs:133-139): out[b·m + pt] = Σ_j c[b·d + j] x^j, m = gridDim.x, for the rows b < rows (blockIdx.y,
+// stepping by gridDim.y).  One CTA per point; thread t owns the coefficients j ≡ t (mod 256) (coalesced), Horner in
+// x^256, then a shared-memory tree sum.  The powers of x are formed once for all the CTA's rows.
 template <class F>
-__global__ void poly_eval_kernel(const F f, const u64* c, size_t d, const u64* xs, u64* out) {
+__global__ void poly_eval_kernel(const F f, const u64* c, size_t d, const u64* xs, u32 rows, u64* out) {
   __shared__ u64 red[256];
   const u32 t = threadIdx.x;
   const u64 x = xs[blockIdx.x];
   const u64 y = field_pow(f, x, 256);
-  u64 acc = 0;
-  if (t < d) {
-    const size_t kmax = (d - 1 - t) / 256;
-    for (size_t k = kmax + 1; k-- > 0;) acc = f.add(f.mul(acc, y), c[t + 256 * k]);
-    acc = f.mul(acc, field_pow(f, x, (u64)t));
-  }
-  red[t] = acc;
-  __syncthreads();
-  for (u32 s = 128; s > 0; s >>= 1) {
-    if (t < s) red[t] = f.add(red[t], red[t + s]);
+  const u64 xt = t < d ? field_pow(f, x, (u64)t) : 0ULL;
+  for (u64 b = blockIdx.y; b < rows; b += gridDim.y) {
+    const u64* cb = c + b * d;
+    u64 acc = 0;
+    if (t < d) {
+      const size_t kmax = (d - 1 - t) / 256;
+      for (size_t k = kmax + 1; k-- > 0;) acc = f.add(f.mul(acc, y), cb[t + 256 * k]);
+      acc = f.mul(acc, xt);
+    }
+    red[t] = acc;
     __syncthreads();
+    for (u32 s = 128; s > 0; s >>= 1) {
+      if (t < s) red[t] = f.add(red[t], red[t + s]);
+      __syncthreads();
+    }
+    if (t == 0) out[b * gridDim.x + blockIdx.x] = red[0];
   }
-  if (t == 0) out[blockIdx.x] = red[0];
 }
 
 // Lagrange-basis evaluate (mod.rs:382-415), literal fold semantics: the closure's early
@@ -341,7 +346,8 @@ static int divrem_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, c
 // enumerates combinations (exponential in K); the value is the unique interpolant, computed here as
 // (1) M by K in-place products, (2) per node j a synthetic division M/(X - x_j) giving q_j and
 // d_j = q_j(x_j) = Π_{k≠j}(x_j - x_k), c_j = y_j/d_j, (3) out = Σ_j c_j q_j with a warp-shuffle
-// reduction per coefficient.  A repeated node gives d_j = 0: the reference's `/` panics → flag.
+// reduction per coefficient.  A repeated node gives d_j = 0: the reference's `/` panics → flag.  Over rows of ys (k
+// words each), blockIdx.y stepping by gridDim.y: d_j^-1 is taken once per node for all the CTA's rows.
 template <class F>
 __global__ void __launch_bounds__(1024)
 interp_master_kernel(const F f, const u64* __restrict__ xs, u32 k, u64* __restrict__ m0, u64* __restrict__ m1) {
@@ -366,7 +372,7 @@ interp_master_kernel(const F f, const u64* __restrict__ xs, u32 k, u64* __restri
 template <class F>
 __global__ void __launch_bounds__(256)
 interp_nodes_kernel(const F f, const u64* __restrict__ M, const u64* __restrict__ xs, const u64* __restrict__ ys, u32 k,
-                    u64* __restrict__ partial /* [ceil(k/32)][k] */, int* flag) {
+                    u32 rows, u64* __restrict__ partial /* [rows][ceil(k/32)][k] */, int* flag) {
   const u32 j = blockIdx.x * blockDim.x + threadIdx.x;
   const bool live = j < k;
   const u64 x = live ? xs[j] : 0ULL;
@@ -376,30 +382,38 @@ interp_nodes_kernel(const F f, const u64* __restrict__ M, const u64* __restrict_
     qv = f.add(M[i], f.mul(qv, x));  // q_j[i-1]
     d = f.add(f.mul(d, x), qv);
   }
-  u64 c = 0;
+  u64 dinv = 0;
   if (live) {
     if (d == 0) atomicExch(flag, 1);
-    else c = f.mul(ys[j], field_pow(f, d, f.modulus() - 2));
+    else dinv = field_pow(f, d, f.modulus() - 2);
   }
-  // pass 2: Σ over the warp's nodes of c_j · q_j[i-1]
+  // pass 2: Σ over the warp's nodes of c_j · q_j[i-1], c_j = y_j / d_j
   const u32 warp = j >> 5, lane = threadIdx.x & 31;
-  qv = 0;
-  for (u32 i = k; i >= 1; i--) {
-    qv = f.add(M[i], f.mul(qv, x));
-    u64 term = f.mul(c, qv);
+  const size_t nwarps = (size_t)gridDim.x * (blockDim.x / 32);
+  for (u64 b = blockIdx.y; b < rows; b += gridDim.y) {
+    const u64 c = live ? f.mul(ys[b * k + j], dinv) : 0ULL;
+    u64* pb = partial + b * nwarps * k;
+    qv = 0;
+    for (u32 i = k; i >= 1; i--) {
+      qv = f.add(M[i], f.mul(qv, x));
+      u64 term = f.mul(c, qv);
 #pragma unroll
-    for (int off = 16; off > 0; off >>= 1) term = f.add(term, __shfl_down_sync(0xFFFFFFFFu, term, off));
-    if (lane == 0) partial[(size_t)warp * k + (i - 1)] = term;
+      for (int off = 16; off > 0; off >>= 1) term = f.add(term, __shfl_down_sync(0xFFFFFFFFu, term, off));
+      if (lane == 0) pb[(size_t)warp * k + (i - 1)] = term;
+    }
   }
 }
 
 template <class F>
-__global__ void interp_sum_kernel(const F f, const u64* __restrict__ partial, u32 k, u32 nwarps, u64* __restrict__ out) {
+__global__ void interp_sum_kernel(const F f, const u64* __restrict__ partial, u32 k, u32 nwarps, u32 rows, u64* __restrict__ out) {
   const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= k) return;
-  u64 acc = 0;
-  for (u32 w = 0; w < nwarps; w++) acc = f.add(acc, partial[(size_t)w * k + i]);
-  out[i] = acc;
+  for (u64 b = blockIdx.y; b < rows; b += gridDim.y) {
+    const u64* pb = partial + b * nwarps * k;
+    u64 acc = 0;
+    for (u32 w = 0; w < nwarps; w++) acc = f.add(acc, pb[(size_t)w * k + i]);
+    out[b * k + i] = acc;
+  }
 }
 
 int poly_mul_schoolbook_rows(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64* b, size_t db, size_t b_stride,
@@ -445,14 +459,20 @@ static int poly_addsub(ronk_ctx* ctx, u64 p, const u64* a, size_t da, const u64*
   });
 }
 
+// poly_eval_kernel over `rows` rows of d coefficients (row b to out + b·m); 1 ≤ m ≤ 2^31 - 1.
+static int poly_eval_rows(ronk_ctx* ctx, u64 p, const u64* c, size_t d, u32 rows, const u64* xs, size_t m, u64* out) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "poly_eval", poly_eval_kernel<std::decay_t<decltype(f)>>, dim3((u32)m, grid_rows(ctx, rows, m)), 256, 0, false, f,
+                  c, d, xs, rows, out);
+  });
+}
+
 int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
   if (!ctx || (m && (!xs || !out)) || (d && !c)) return set_err(ctx, RONK_EINVAL, "null argument");
   RONK_TRY(validate_modulus(ctx, p));
   if (m == 0) return RONK_OK;
   if (m > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "too many points");
-  return with_field(ctx, p, 0, false, [&](const auto& f) {
-    return launch(ctx, "poly_eval", poly_eval_kernel<std::decay_t<decltype(f)>>, (u32)m, 256, 0, false, f, c, d, xs, out);
-  });
+  return poly_eval_rows(ctx, p, c, d, 1, xs, m, out);
 }
 
 // nodes[i] = ω_n^i (plain residues)
@@ -469,9 +489,10 @@ int roots_table(ronk_ctx* ctx, u64 p, u64 g, u64 n, u64* nodes) {
   });
 }
 
-// The literal interpolation (interp_* kernels above) through k ≤ 8192 nodes into out; scratch m0 and m1 of k + 1 words,
-// partial of ⌈k/256⌉·8·k words.  Synchronous; RONK_EINVAL for a repeated x, with out written.
-static int interp_literal(ronk_ctx* ctx, u64 p, const u64* X, const u64* Y, size_t k, u64* out, u64* m0, u64* m1,
+// The literal interpolation (interp_* kernels above) of `rows` rows of Y (k words each) through k ≤ 8192 nodes into out;
+// scratch m0 and m1 of k + 1 words, partial of rows·⌈k/256⌉·8·k words.  Synchronous; RONK_EINVAL for a repeated x, with
+// out written.
+static int interp_literal(ronk_ctx* ctx, u64 p, const u64* X, const u64* Y, size_t k, u32 rows, u64* out, u64* m0, u64* m1,
                           u64* partial) {
   const u32 blocks = ((u32)k + 255) / 256, nwarps = blocks * 8;
   RONK_TRY(reset_flag(ctx));
@@ -479,9 +500,10 @@ static int interp_literal(ronk_ctx* ctx, u64 p, const u64* X, const u64* Y, size
     using F = std::decay_t<decltype(f)>;
     RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, X, (u32)k, m0, m1));
     const u64* M = (k & 1) ? m1 : m0;
-    RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, blocks, 256, 0, false, f, M, X, Y, (u32)k, partial,
-                    ctx->d_flag));
-    return launch(ctx, "interp_sum", interp_sum_kernel<F>, blocks, 256, 0, false, f, partial, (u32)k, nwarps, out);
+    RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, dim3(blocks, grid_rows(ctx, rows, blocks)), 256, 0, false, f, M, X, Y,
+                    (u32)k, rows, partial, ctx->d_flag));
+    return launch(ctx, "interp_sum", interp_sum_kernel<F>, dim3(blocks, grid_rows(ctx, rows, blocks)), 256, 0, false, f, partial, (u32)k,
+                  nwarps, rows, out);
   }));
   int v = 0;
   RONK_TRY(read_flag(ctx, &v));
@@ -500,6 +522,24 @@ constexpr size_t kInterpTreeMin = 2048;       // k (1.13 vs 1.89 ms; 1024: 1.25 
 
 static size_t tree_min(const ronk_ctx* ctx, size_t measured) {
   return ctx->tune.tree_min >= 0 ? (size_t)ctx->tune.tree_min : measured;
+}
+
+// Batches of rows over one point set (tools/multipoint_batch_timing.py on an H100 80GB HBM3 at 700 W, DESIGN.md §5, at
+// batch 1, 2, 16 and 256): the literal kernels cost about batch·n² (n = min(d, m) or k) and, at small n, a fixed amount per
+// row and point, while the tree's cost barely grows with the batch.  Multieval takes the tree from batch·n² ≥ 2^30 (at
+// batch 1 the single-row n ≥ 2^15; 16 rows from n = 8192: 1.41 vs 1.92 ms, 4096: 1.17 vs 0.56) or batch·n ≥ 2^18 (256
+// rows from n = 1024: 0.82 vs 0.83 ms, 2048: 0.99 vs 2.52); interpolation from k ≥ 2048 as for one row, or batch·k² ≥
+// 2^28 (256 rows from k = 1024: 1.19 vs 2.60 ms; 512: 0.79 vs 0.79).  RONK_TREE_MIN overrides both, whatever the batch.
+static bool multieval_takes_tree(const ronk_ctx* ctx, size_t n, u32 batch) {
+  if (ctx->tune.tree_min >= 0) return n >= (size_t)ctx->tune.tree_min;
+  static_assert(kMultievalTreeMin == (size_t)1 << 15, "batch·n² ≥ 2^30 is n ≥ kMultievalTreeMin at batch 1");
+  const u64 n64 = n, b = batch;
+  return n64 >= kMultievalTreeMin || n64 * n64 >= (((u64)1 << 30) + b - 1) / b || b * n64 >= ((u64)1 << 18);  // n ≤ 2^24
+}
+static bool interp_takes_tree(const ronk_ctx* ctx, size_t k, u32 batch) {
+  if (ctx->tune.tree_min >= 0) return k >= (size_t)ctx->tune.tree_min;
+  const u64 k64 = k;
+  return k64 >= kInterpTreeMin || k64 * k64 >= (((u64)1 << 28) + batch - 1) / batch;  // k ≤ 2^24
 }
 
 // Checks shared by the three: RONK_EINVAL for a null pointer or g out of range, RONK_EUNSUPPORTED above 2^24 points.
@@ -534,32 +574,78 @@ static int from_roots_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t 
   });
 }
 
-static int multieval_device(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u64* xs, size_t m, u64* out) {
-  RONK_TRY(tree_args(ctx, p, g, m, (m && (!xs || !out)) || (d && !c)));
-  if (m == 0) return RONK_OK;
-  if (overlaps(out, m, xs, m) || overlaps(out, m, c, d)) return set_err(ctx, RONK_EINVAL, "out may not overlap coeffs or xs");
-  if (d && tree_fits(p, g, m, d) && std::min(d, m) >= tree_min(ctx, kMultievalTreeMin))
-    return tree_multieval(ctx, p, g, c, d, xs, m, out);
-  return poly_eval_device(ctx, p, c, d, xs, m, out);
+// The batched entries' envelope: batch·N words in each row buffer of the tree, N = 2^⌈log2 size⌉ (for multieval also
+// the root's 2^⌈log2(2d - 1)⌉), as ronk_poly_mul_batch_u64's batched transforms; batch·⌈k/256⌉·8·k words of the literal
+// interpolation's per-warp partial sums.
+constexpr u64 kTreeBatchMaxWords = (u64)1 << 32;
+
+// The single-row entries are batch = 1 without `reserve`; the batched ones take all the call's scratch before the first
+// launch (reserve), so that what follows fits the blocks that take leaves.
+static int reserve_scratch(ronk_ctx* ctx, size_t words) {
+  Frame fr(ctx);
+  u64* all = nullptr;
+  return fr.take(&all, words);
 }
 
-static int interpolate_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u64* out) {
-  RONK_TRY(tree_args(ctx, p, g, k, k && (!xs || !ys || !out)));
-  if (k == 0) return RONK_OK;
-  if (overlaps(out, k, xs, k) || overlaps(out, k, ys, k)) return set_err(ctx, RONK_EINVAL, "out may not overlap xs or ys");
-  if (tree_fits(p, g, k, k) && (k >= tree_min(ctx, kInterpTreeMin) || k > kInterpLiteralMax))
-    return tree_interpolate(ctx, p, g, xs, ys, k, out);
+// The path of a non-empty call and the checks that go with it, which read no pointer, so that the _host twins make them
+// before they stage anything: *tree, or RONK_EUNSUPPORTED past the envelope.
+static int multieval_path(ronk_ctx* ctx, u64 p, u64 g, size_t d, u32 batch, size_t m, bool* tree) {
+  *tree = d && tree_fits(p, g, m, d) && multieval_takes_tree(ctx, std::min(d, m), batch);
+  if (!*tree) return RONK_OK;
+  const u64 N = std::max((u64)1 << log2_ceil(m), (u64)1 << std::max<u32>(1, log2_ceil(2 * d - 1)));
+  if ((u64)batch * N > kTreeBatchMaxWords) return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^32 words of tree rows");
+  return RONK_OK;
+}
+
+static int interpolate_path(ronk_ctx* ctx, u64 p, u64 g, size_t k, u32 batch, bool* tree) {
+  *tree = tree_fits(p, g, k, k) && (interp_takes_tree(ctx, k, batch) || k > kInterpLiteralMax);
+  if (*tree) {
+    if ((u64)batch << log2_ceil(k) > kTreeBatchMaxWords)
+      return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^32 words of tree rows");
+    return RONK_OK;
+  }
   if (k > kInterpLiteralMax)
     return set_err(ctx, RONK_EUNSUPPORTED, "more than 8192 nodes off the tree path (O(K²) interpolation)");
+  if ((u64)batch * ((k + 255) / 256 * 8) * k > kTreeBatchMaxWords)
+    return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^32 words of per-warp partial sums");
+  return RONK_OK;
+}
+
+static int multieval_device(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, u32 batch, const u64* xs, size_t m, u64* out,
+                            bool reserve) {
+  RONK_TRY(tree_args(ctx, p, g, m, (m && (!xs || !out)) || (d && !c)));
+  if (m == 0 || batch == 0) return RONK_OK;
+  if (d > ~(u64)0 / batch) return set_err(ctx, RONK_EUNSUPPORTED, "batch·d words overflow");
+  const size_t nc = (size_t)batch * d, no = (size_t)batch * m;
+  if (overlaps(out, no, xs, m) || overlaps(out, no, c, nc)) return set_err(ctx, RONK_EINVAL, "out may not overlap coeffs or xs");
+  bool tree = false;
+  RONK_TRY(multieval_path(ctx, p, g, d, batch, m, &tree));
+  if (!tree) return poly_eval_rows(ctx, p, c, d, batch, xs, m, out);
+  if (reserve) RONK_TRY(reserve_scratch(ctx, tree_scratch_words(ctx, m, d, batch, false)));
+  return tree_multieval(ctx, p, g, c, d, batch, xs, m, out);
+}
+
+static int interpolate_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u32 batch, u64* out,
+                              bool reserve) {
+  RONK_TRY(tree_args(ctx, p, g, k, k && (!xs || !ys || !out)));
+  if (k == 0 || batch == 0) return RONK_OK;
+  const size_t ny = (size_t)batch * k;
+  if (overlaps(out, ny, xs, k) || overlaps(out, ny, ys, ny)) return set_err(ctx, RONK_EINVAL, "out may not overlap xs or ys");
+  bool tree = false;
+  RONK_TRY(interpolate_path(ctx, p, g, k, batch, &tree));
+  if (tree) {
+    if (reserve) RONK_TRY(reserve_scratch(ctx, tree_scratch_words(ctx, k, k, batch, true)));
+    return tree_interpolate(ctx, p, g, xs, ys, k, batch, out);
+  }
   // the literal kernels into scratch, so that a repeated x leaves out unwritten
   const size_t nwarps = (k + 255) / 256 * 8;
   Frame fr(ctx);
   u64* res = nullptr;
-  RONK_TRY(fr.take(&res, 3 * k + 2 + nwarps * k));
-  u64* m0 = res + k;
+  RONK_TRY(fr.take(&res, ny + 2 * (k + 1) + batch * nwarps * k));
+  u64* m0 = res + ny;
   u64* m1 = m0 + k + 1;
-  RONK_TRY(interp_literal(ctx, p, xs, ys, k, res, m0, m1, m1 + k + 1));
-  RONK_CUDA(ctx, cudaMemcpyAsync(out, res, k * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
+  RONK_TRY(interp_literal(ctx, p, xs, ys, k, batch, res, m0, m1, m1 + k + 1));
+  RONK_CUDA(ctx, cudaMemcpyAsync(out, res, ny * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return RONK_OK;
 }
@@ -695,7 +781,7 @@ int ronk_poly_interpolate_u64_host(ronk_ctx* ctx, uint64_t p, const uint64_t* xs
   Staged s[] = {{k * 8, xs}, {k * 8, ys}, {k * 8, nullptr, out}, {(k + 1) * 8}, {(k + 1) * 8}, {nwarps * k * 8}};
   Frame fr(ctx);
   RONK_TRY(stage_in(fr, s));
-  RONK_TRY(interp_literal(ctx, p, s[0].dev, s[1].dev, k, s[2].dev, s[3].dev, s[4].dev, s[5].dev));
+  RONK_TRY(interp_literal(ctx, p, s[0].dev, s[1].dev, k, 1, s[2].dev, s[3].dev, s[4].dev, s[5].dev));
   return stage_out(ctx, RONK_OK, s);
 }
 
@@ -707,13 +793,54 @@ int ronk_poly_from_roots_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64
 int ronk_poly_multieval_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* coeffs, size_t d, const uint64_t* xs,
                             size_t m, uint64_t* out) {
   ronk::DeviceGuard _dg(ctx);
-  return multieval_device(ctx, p, g, (const u64*)coeffs, d, (const u64*)xs, m, (u64*)out);
+  return multieval_device(ctx, p, g, (const u64*)coeffs, d, 1, (const u64*)xs, m, (u64*)out, false);
 }
 
 int ronk_poly_interpolate_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, const uint64_t* ys, size_t k,
                               uint64_t* out) {
   ronk::DeviceGuard _dg(ctx);
-  return interpolate_device(ctx, p, g, (const u64*)xs, (const u64*)ys, k, (u64*)out);
+  return interpolate_device(ctx, p, g, (const u64*)xs, (const u64*)ys, k, 1, (u64*)out, false);
+}
+
+int ronk_poly_multieval_batch_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* coeffs, size_t d, uint32_t batch,
+                                  const uint64_t* xs, size_t m, uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  return multieval_device(ctx, p, g, (const u64*)coeffs, d, batch, (const u64*)xs, m, (u64*)out, true);
+}
+
+int ronk_poly_interpolate_batch_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, const uint64_t* ys, size_t k,
+                                    uint32_t batch, uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  return interpolate_device(ctx, p, g, (const u64*)xs, (const u64*)ys, k, batch, (u64*)out, true);
+}
+
+// Host pointers: the device function's checks that read no pointer, and its size checks, come first, so that nothing is
+// staged for an empty call or one refused for its arguments or its size.
+int ronk_poly_multieval_batch_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* coeffs, size_t d, uint32_t batch,
+                                       const uint64_t* xs, size_t m, uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  RONK_TRY(tree_args(ctx, p, g, m, (m && (!xs || !out)) || (d && !coeffs)));
+  if (m == 0 || batch == 0) return RONK_OK;
+  if (d > ~(u64)0 / 8 / batch) return set_err(ctx, RONK_EUNSUPPORTED, "batch·d words overflow");
+  bool tree = false;
+  RONK_TRY(multieval_path(ctx, p, g, d, batch, m, &tree));
+  Staged s[] = {{(size_t)batch * d * 8, coeffs}, {m * 8, xs}, {(size_t)batch * m * 8, nullptr, out}};
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
+  return stage_out(ctx, multieval_device(ctx, p, g, s[0].dev, d, batch, s[1].dev, m, s[2].dev, true), s);
+}
+
+int ronk_poly_interpolate_batch_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, const uint64_t* ys,
+                                         size_t k, uint32_t batch, uint64_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  RONK_TRY(tree_args(ctx, p, g, k, k && (!xs || !ys || !out)));
+  if (k == 0 || batch == 0) return RONK_OK;
+  bool tree = false;
+  RONK_TRY(interpolate_path(ctx, p, g, k, batch, &tree));
+  Staged s[] = {{k * 8, xs}, {(size_t)batch * k * 8, ys}, {(size_t)batch * k * 8, nullptr, out}};
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
+  return stage_out(ctx, interpolate_device(ctx, p, g, s[0].dev, s[1].dev, k, batch, s[2].dev, true), s);
 }
 
 // ronk_poly_divrem_u64 with g = 0 (no Newton path) on staged copies of a and b.  Its checks up to da == 0 run before

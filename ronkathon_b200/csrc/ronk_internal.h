@@ -459,8 +459,21 @@ int newton_inverse_device(ronk_ctx* ctx, u64 p, u64 g, const u64* hr, size_t hl,
 constexpr size_t kTreeLeaves = 64, kTreeMaxLeaves = (size_t)1 << 24;
 bool tree_fits(u64 p, u64 g, size_t k, size_t d);
 int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out);
-int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, const u64* xs, size_t m, u64* out);
-int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u64* out);
+// multieval and interpolate take `batch` rows over the one point set (c: batch × d, ys and out row-major); batch 1 is the
+// single-row launch sequence.  tree_scratch_words: an upper bound on the words either takes from the context's scratch,
+// its transforms' workspace included.
+int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, u32 batch, const u64* xs, size_t m, u64* out);
+int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u32 batch, u64* out);
+size_t tree_scratch_words(const ronk_ctx* ctx, size_t k, size_t d, u32 batch, bool interp);
+// grid.y of a kernel whose grid_x CTAs step over `rows` rows by gridDim.y: enough rows of CTAs to give every SM 8 (at
+// least one row, at most `rows` and CUDA's 65535), so that each CTA serves several rows of a large batch and forms what
+// the rows share once for all of them.
+inline u32 grid_rows(const ronk_ctx* ctx, u64 rows, u64 grid_x) {
+  const u64 fill = ((u64)ctx->sm_count * 8 + grid_x - 1) / grid_x;
+  u64 y = rows < fill ? rows : fill;
+  if (y > 65535) y = 65535;
+  return y ? (u32)y : 1u;
+}
 // ntt_any.cu: ronk_ntt_any_u64 on device pointers, and its argument and path check (*path set on RONK_OK).
 enum AnyNttPath { AN_POW2, AN_BLUESTEIN, AN_LITERAL, AN_NONE };
 int anyntt_args(ronk_ctx* ctx, u64 p, u64 g, const void* data, u64 n, AnyNttPath* path);

@@ -176,6 +176,30 @@ def poly_interpolate(ctx: Context, xs, ys, p: int = GOLDILOCKS, g: int = 7):
     return out
 
 
+def poly_multieval_batch(ctx: Context, coeffs, xs, p: int = GOLDILOCKS, g: int = 7):
+    """evaluate every row of coeffs (batch, d) at every xs[i]: a new (batch, m) tensor, row b the words poly_multieval
+    gives for coeffs[b].  One subproduct tree over xs serves every row.  Asynchronous."""
+    import torch
+    _check_u64(coeffs); _check_u64(xs)
+    assert coeffs.dim() == 2, "coeffs is (batch, d)"
+    batch, d = coeffs.shape
+    out = torch.empty((batch, xs.numel()), dtype=torch.int64, device=xs.device)
+    ctx.call("ronk_poly_multieval_batch_u64", p, g, _lib._ptr(coeffs), d, batch, _lib._ptr(xs), xs.numel(), _lib._ptr(out))
+    return out
+
+
+def poly_interpolate_batch(ctx: Context, xs, ys, p: int = GOLDILOCKS, g: int = 7):
+    """The interpolant through (xs[i], ys[b, i]) for every row of ys (batch, k): a new (batch, k) tensor, row b the words
+    poly_interpolate gives for ys[b].  One subproduct tree over xs serves every row.  Synchronous; raises RonkPanic for
+    a repeated x."""
+    import torch
+    _check_u64(xs); _check_u64(ys)
+    assert ys.dim() == 2 and ys.shape[1] == xs.numel(), "ys is (batch, len(xs))"
+    out = torch.empty_like(ys)
+    ctx.call("ronk_poly_interpolate_batch_u64", p, g, _lib._ptr(xs), _lib._ptr(ys), xs.numel(), ys.shape[0], _lib._ptr(out))
+    return out
+
+
 def rs_encode(ctx: Context, msg, n: int, batch: int = 1, p: int = GOLDILOCKS, g: int = 7):
     """Reed–Solomon Message::encode of `batch` messages (msg: batch × k, row-major): a new batch × n tensor of
     codewords, position i holding the message polynomial at ω_n^i."""
