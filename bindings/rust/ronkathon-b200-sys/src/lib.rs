@@ -112,6 +112,8 @@ extern "C" {
   pub fn ronk_rs_encode_u64(ctx: *mut ronk_ctx, p: u64, g: u64, msg: *const u64, k: u64, n: u64, batch: u32, codeword: *mut u64) -> c_int;
   pub fn ronk_rs_decode_u64(ctx: *mut ronk_ctx, p: u64, g: u64, received: *const u64, erased: *const u8, n: u64, k: u64, batch: u32, msg: *mut u64, status: *mut i32) -> c_int;
   pub fn ronk_rs_decode_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, received: *const u64, erased: *const u8, n: u64, k: u64, batch: u32, msg: *mut u64, status: *mut i32) -> c_int;
+  pub fn ronk_rs_decode_at_u64(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, received: *const u64, erased: *const u8, n: u64, k: u64, batch: u32, msg: *mut u64, status: *mut i32) -> c_int;
+  pub fn ronk_rs_decode_at_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, xs: *const u64, received: *const u64, erased: *const u8, n: u64, k: u64, batch: u32, msg: *mut u64, status: *mut i32) -> c_int;
 
   // AffinePoint<PlutoExtendedCurve> + kzg::commit (src/curve/mod.rs:157-235, src/kzg/setup.rs:48-60)
   pub fn ronk_point_add_pluto_ext_host(ctx: *mut ronk_ctx, a: *const u8, b: *const u8, out: *mut u8, n: usize) -> c_int;

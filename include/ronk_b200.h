@@ -419,6 +419,34 @@ int ronk_rs_decode_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *re
                        uint64_t k, uint32_t batch, uint64_t *msg, int32_t *status);
 int ronk_rs_decode_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *received, const uint8_t *erased,
                             uint64_t n, uint64_t k, uint32_t batch, uint64_t *msg, int32_t *status);
+/* Errors-and-erasures decoding of `batch` received words (batch × n) whose positions share any n distinct points xs
+ * (canonical residues; 0 is allowed): row b is meant to be f_b(xs[i]) for an f_b of degree < k, for example Shamir
+ * shares at x = 1..n.  erased, msg, status and the guarantee are those of ronk_rs_decode_u64: within 2e + ε ≤ n - k
+ * msg[b] = f_b and status[b] = e; otherwise -1 with a zero message, or a message whose evaluations differ from the row
+ * in e' non-erased positions, 2e' + ε ≤ n - k.  The values at erased positions are never read.  At xs[i] = ω_n^i this
+ * gives ronk_rs_decode_u64's words, beyond the radius too.
+ * Steps, with m = n - k and M = Π (X - x_i): the interpolant of each row (erasures zeroed) gives the syndromes
+ * S_j = Σ_i r_i·x_i^j / M'(x_i) through one product with 1 / (z^n·M(1/z)) mod z^m (ronk_poly_divrem_u64's quotient);
+ * the Berlekamp–Massey locator of ronk_rs_decode_u64; one batched multieval of the 3·batch locator rows (m + 1 words)
+ * and one of M' over xs; Forney's e_i = Ω̂(x_i)·M'(x_i)/σ'(x_i) at the roots; a second batched interpolation and the
+ * check that it has degree < k.  Each step takes its entry point's path: the subproduct tree up to 2^24 points, the
+ * literal kernels up to 8192; g = 0 keeps every step on the literal kernels.
+ * Errors, in this order: RONK_EINVAL for a null pointer (xs, received, msg, status), a bad modulus, g >= p, n == 0, k == 0
+ * or k > n; RONK_EUNSUPPORTED for n - k > RONK_RS_MAX_PARITY, n > 2^24, 3·batch ≥ 2^32, past the envelope of
+ * ronk_poly_interpolate_batch_u64 over batch rows or of ronk_poly_multieval_batch_u64 over 3·batch rows of n - k + 1
+ * words, or batch·2^⌈log2(2(n - k) - 1)⌉ > 2^32; then RONK_EINVAL for an output that overlaps an input, and for a
+ * repeated point (found by the first interpolation, before anything is written).  batch == 0 does nothing.  Nothing is
+ * written to msg or status on any error.
+ * Scratch: 8·(batch·(5n + 6(n - k) + 4) + 6n + 4(n - k) + 1) bytes, with above it the largest that one step's entry
+ * point takes: the batched interpolation's over batch rows, the batched multieval's over 3·batch rows, ronk_poly_divrem_u64's
+ * of n + m words by n + 1 and ronk_poly_mul_batch_u64's of batch rows of n - k words by one shared row.
+ * The call synchronises with the host: each interpolation reads its repeated-node flag and the division reads the
+ * divisor's top word.  The _host variant makes every check above but the repeated point before it stages anything,
+ * refuses a point x >= p with RONK_EINVAL, stages in and out and synchronises. */
+int ronk_rs_decode_at_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *received,
+                          const uint8_t *erased, uint64_t n, uint64_t k, uint32_t batch, uint64_t *msg, int32_t *status);
+int ronk_rs_decode_at_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *xs, const uint64_t *received,
+                               const uint8_t *erased, uint64_t n, uint64_t k, uint32_t batch, uint64_t *msg, int32_t *status);
 
 /* ---- curve + kzg::commit ------------------------------------------------------------------ */
 /* AffinePoint Add / Neg / Mul<ScalarField> — src/curve/mod.rs:178-213, :225-235, :157-172,

@@ -90,6 +90,8 @@ SIGNATURES = {
     "ronk_rs_encode_u64": (i32, [vp, u64, u64, vp, u64, u64, u32, vp]),
     "ronk_rs_decode_u64": (i32, [vp, u64, u64, vp, vp, u64, u64, u32, vp, vp]),
     "ronk_rs_decode_u64_host": (i32, [vp, u64, u64, vp, vp, u64, u64, u32, vp, vp]),
+    "ronk_rs_decode_at_u64": (i32, [vp, u64, u64, vp, vp, vp, u64, u64, u32, vp, vp]),
+    "ronk_rs_decode_at_u64_host": (i32, [vp, u64, u64, vp, vp, vp, u64, u64, u32, vp, vp]),
     "ronk_point_add_pluto_ext_host": (i32, [vp, vp, vp, vp, sz]),
     "ronk_point_neg_pluto_ext_host": (i32, [vp, vp, vp, sz]),
     "ronk_point_smul_pluto_ext_host": (i32, [vp, vp, vp, vp, sz]),

@@ -10,6 +10,8 @@
 * Shamir `split` (src/shamir/mod.rs:53-58): `Polynomial::evaluate` at x = 1..n, one batched kernel.
 * Shamir `split_secret` / `combine_shares` over batches of secrets (`shamir_split`, `shamir_combine`): one batched
   multipoint evaluation at x = 1..n, and one batched interpolation through the shares' x's.
+* Shamir recovery from wrong or missing shares (`shamir_recover`): errors-and-erasures Reed–Solomon decoding of every
+  row at the shares' x's (`ronk_rs_decode_at_u64_host`).
 """
 from __future__ import annotations
 
@@ -123,3 +125,32 @@ def shamir_combine(shares_xs, shares_ys, field):
         _lib.default_context().call("ronk_poly_interpolate_batch_u64_host", p, field.PRIMITIVE_ELEMENT.value,
                                     _lib._ptr(xs), _lib._ptr(ys), k, len(ys), _lib._ptr(out))
     return [field(int(v)) for v in out[:, 0]]
+
+
+def shamir_recover(shares_xs, shares_ys, threshold: int, field, missing=None):
+    """combine_shares that survives dishonest and absent shareholders: shares_xs (n,) are the distinct x's every
+    secret's shares share, shares_ys is (batch, n), and `missing` (None, or a (batch, n) mask) marks shares known to be
+    absent, whose y's are never read.  Every row is Reed–Solomon decoded at the x's, with message length `threshold`:
+    with e wrong and ε missing shares, a row with 2e + ε ≤ n - threshold gives its secret exactly.  Returns
+    (secrets, errors): a secret is a field element, or None for a row that cannot be recovered (then errors is -1);
+    errors[b] counts the wrong shares found in row b.  No row is ever given a secret whose polynomial differs from its
+    shares in more than (n - threshold - ε)/2 of them.  One batched device decode (ronk_rs_decode_at_u64_host); a
+    repeated x panics (RonkPanic)."""
+    from . import _lib
+    p = field.ORDER
+    xs = np.array([int(getattr(x, "value", x)) % p for x in shares_xs], dtype=np.uint64)
+    n = len(xs)
+    assert 0 < threshold <= n, "need 0 < threshold <= share count"
+    ys = np.array([[int(getattr(y, "value", y)) % p for y in row] for row in shares_ys], dtype=np.uint64).reshape(-1, n)
+    batch = len(ys)
+    erased = None
+    if missing is not None:
+        erased = np.ascontiguousarray(np.asarray(missing, dtype=bool).reshape(batch, n), dtype=np.uint8)
+    msg = np.empty((batch, threshold), dtype=np.uint64)
+    status = np.empty(batch, dtype=np.int32)
+    if batch:
+        _lib.default_context().call("ronk_rs_decode_at_u64_host", p, field.PRIMITIVE_ELEMENT.value, _lib._ptr(xs),
+                                    _lib._ptr(ys), _lib._ptr(erased), n, threshold, batch, _lib._ptr(msg),
+                                    _lib._ptr(status))
+    secrets = [field(int(msg[b, 0])) if status[b] >= 0 else None for b in range(batch)]
+    return secrets, [int(s) for s in status]

@@ -589,7 +589,7 @@ static int reserve_scratch(ronk_ctx* ctx, size_t words) {
 
 // The path of a non-empty call and the checks that go with it, which read no pointer, so that the _host twins make them
 // before they stage anything: *tree, or RONK_EUNSUPPORTED past the envelope.
-static int multieval_path(ronk_ctx* ctx, u64 p, u64 g, size_t d, u32 batch, size_t m, bool* tree) {
+int multieval_path(ronk_ctx* ctx, u64 p, u64 g, size_t d, u32 batch, size_t m, bool* tree) {
   *tree = d && tree_fits(p, g, m, d) && multieval_takes_tree(ctx, std::min(d, m), batch);
   if (!*tree) return RONK_OK;
   const u64 N = std::max((u64)1 << log2_ceil(m), (u64)1 << std::max<u32>(1, log2_ceil(2 * d - 1)));
@@ -597,7 +597,7 @@ static int multieval_path(ronk_ctx* ctx, u64 p, u64 g, size_t d, u32 batch, size
   return RONK_OK;
 }
 
-static int interpolate_path(ronk_ctx* ctx, u64 p, u64 g, size_t k, u32 batch, bool* tree) {
+int interpolate_path(ronk_ctx* ctx, u64 p, u64 g, size_t k, u32 batch, bool* tree) {
   *tree = tree_fits(p, g, k, k) && (interp_takes_tree(ctx, k, batch) || k > kInterpLiteralMax);
   if (*tree) {
     if ((u64)batch << log2_ceil(k) > kTreeBatchMaxWords)

@@ -263,7 +263,7 @@ static int spread(ronk_ctx* ctx, const u64* src, size_t stride, size_t len, u32 
                 A, B);
 }
 
-static int reverse_rows(ronk_ctx* ctx, const u64* src, size_t ss, size_t last, size_t n, u64* dst, size_t ds, size_t len,
+int reverse_rows(ronk_ctx* ctx, const u64* src, size_t ss, size_t last, size_t n, u64* dst, size_t ds, size_t len,
                         u32 batch) {
   const size_t total = (size_t)batch * len;
   return launch(ctx, "tree_reverse", tree_reverse_rows_kernel, grid_for(ctx, total, 256), 256, 0, false, src, ss, last, n, dst,
@@ -371,6 +371,13 @@ size_t tree_scratch_words(const ronk_ctx* ctx, size_t k, size_t d, u32 batch, bo
   size_t above = std::max((size_t)batch * t.N, nq);
   if (!interp && batch > 1) above = std::max(above, poly_mul_rows_pow2_scratch(ctx, d, d + 1, true, batch));
   return tree + root + above + 16 * Frame::kAlign / 8;  // and each take's rounding to 256 bytes
+}
+
+int poly_deriv(ronk_ctx* ctx, u64 p, const u64* M, size_t k, u64* out) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "tree_deriv", tree_deriv_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, k, 256), 256, 0, false, f, M, k,
+                  out);
+  });
 }
 
 int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* out) {

@@ -465,6 +465,14 @@ int tree_from_roots(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t k, u64* o
 int tree_multieval(ronk_ctx* ctx, u64 p, u64 g, const u64* c, size_t d, u32 batch, const u64* xs, size_t m, u64* out);
 int tree_interpolate(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* ys, size_t k, u32 batch, u64* out);
 size_t tree_scratch_words(const ronk_ctx* ctx, size_t k, size_t d, u32 batch, bool interp);
+// poly_tree.cu: reverse_words over `batch` rows, dst[b·ds + i] = i < n ? src[b·ss + last - i] : 0, i < len, one launch
+// profiled as tree_reverse; out[i] = (i + 1)·M[i + 1], i < k, one launch profiled as tree_deriv.
+int reverse_rows(ronk_ctx* ctx, const u64* src, size_t ss, size_t last, size_t n, u64* dst, size_t ds, size_t len, u32 batch);
+int poly_deriv(ronk_ctx* ctx, u64 p, const u64* M, size_t k, u64* out);
+// poly.cu: the path of a non-empty batched multieval / interpolation (*tree) and its size checks, which read no
+// pointer: RONK_EUNSUPPORTED past the envelope of ronk_poly_multieval_batch_u64 / ronk_poly_interpolate_batch_u64.
+int multieval_path(ronk_ctx* ctx, u64 p, u64 g, size_t d, u32 batch, size_t m, bool* tree);
+int interpolate_path(ronk_ctx* ctx, u64 p, u64 g, size_t k, u32 batch, bool* tree);
 // grid.y of a kernel whose grid_x CTAs step over `rows` rows by gridDim.y: enough rows of CTAs to give every SM 8 (at
 // least one row, at most `rows` and CUDA's 65535), so that each CTA serves several rows of a large batch and forms what
 // the rows share once for all of them.

@@ -43,13 +43,18 @@ __device__ __forceinline__ u64 rs_warp_sum(const F& f, u64 v) {
   return v;
 }
 
-// One CTA per row.  Y: the rows' scaled inverse transforms (batch × n); erased: batch × n bytes or null; winv = ω^-1.
-// Writes, for row b, Ψ, Ψ' and Ω zero-padded to `ld` words at out + b·ld, + plane + b·ld, + 2·plane + b·ld (all zero
-// for a failed row), and rows[b].  Thread t owns the coefficients i = t + j·blockDim.x, j < RS_LOC_PER.
-template <class F>
-__global__ void __launch_bounds__(RS_LOC_MAX_THREADS)
-rs_locator_kernel(const F f, const u64* __restrict__ Y, const uint8_t* __restrict__ erased, u64 n, u64 k, u64 winv,
-                  u64* __restrict__ out, u64 ld, u64 plane, RsRow* __restrict__ rows) {
+// The locator of one row per CTA, for both decoders.  AT = false (ronk_rs_decode_u64): the syndromes are
+// Y[b·n + k + j] of the rows' scaled inverse transforms, the erasure at position i contributes (1 - ω^-i z), and the
+// outputs are Ψ, Ψ', Ω with rows[b].deg = deg Ψ.  AT = true (ronk_rs_decode_at_u64): the syndromes are Y[b·sld + j],
+// the erasure at position i contributes (1 - xs[i]·z), and the outputs are the reversed forms σ = X^L·Ψ(1/X), σ' and
+// Ω̂ = X^(L-1)·Ω(1/X) with rows[b].deg = L, Berlekamp–Massey's length: a point at 0 adds the factor 1 to Ψ but a root
+// at 0 to σ, so deg Ψ would miss it.  Either way the outputs are zero-padded to `ld` words at out + b·ld,
+// + plane + b·ld, + 2·plane + b·ld (all zero for a failed row).  Thread t owns the coefficients i = t + j·blockDim.x,
+// j < RS_LOC_PER.
+template <class F, bool AT>
+__device__ __forceinline__ void rs_locator_body(const F& f, const u64* __restrict__ Y, u64 sld, const u64* __restrict__ xs,
+                                                const uint8_t* __restrict__ erased, u64 n, u64 k, u64 winv,
+                                                u64* __restrict__ out, u64 ld, u64 plane, RsRow* __restrict__ rows) {
   extern __shared__ u64 sm[];
   __shared__ u64 red[2][RS_LOC_MAX_THREADS / 32];
   __shared__ u32 count;
@@ -64,12 +69,16 @@ rs_locator_kernel(const F f, const u64* __restrict__ Y, const uint8_t* __restric
     top = 0;
   }
   __syncthreads();
-  // the erasures' ω^-i, in any order (Γ is a product), into S's space: S is loaded after Γ is built
+  // the erasures' ω^-i (x_i), in any order (Γ is a product), into S's space: S is loaded after Γ is built
   if (erased)
     for (u64 i = t; i < n; i += T)
       if (erased[b * n + i]) {
         const u32 at = atomicAdd(&count, 1u);
-        if (at < m) S[at] = field_pow(f, winv, i);
+        if constexpr (AT) {
+          if (at < m) S[at] = xs[i];
+        } else {
+          if (at < m) S[at] = field_pow(f, winv, i);
+        }
       }
   for (u64 i = t; i <= m; i += T) Bb(0)[i] = i == 0 ? 1 % f.modulus() : 0;
   __syncthreads();
@@ -93,7 +102,11 @@ rs_locator_kernel(const F f, const u64* __restrict__ Y, const uint8_t* __restric
     psi[j] = !fail && i <= m ? Bb(cur)[i] : 0;
   }
   __syncthreads();  // the erasure list is read; S may be loaded
-  for (u64 j = t; j < m; j += T) S[j] = Y[b * n + k + j];
+  if constexpr (AT) {
+    for (u64 j = t; j < m; j += T) S[j] = Y[b * sld + j];
+  } else {
+    for (u64 j = t; j < m; j += T) S[j] = Y[b * n + k + j];
+  }
   __syncthreads();
   if (!fail) {
     // Berlekamp–Massey, one barrier per step: Ψ stays in registers, B is read at Bb(cur) and a new B written to the
@@ -139,10 +152,14 @@ rs_locator_kernel(const F f, const u64* __restrict__ Y, const uint8_t* __restric
         s++;
       }
     }
+    if constexpr (AT) {
+      if (t == 0) top = (int)L;
+    } else {
 #pragma unroll
-    for (int j = 0; j < RS_LOC_PER; j++) {
-      const u64 i = t + (u64)j * T;
-      if (i <= m && psi[j]) atomicMax(&top, (int)i);
+      for (int j = 0; j < RS_LOC_PER; j++) {
+        const u64 i = t + (u64)j * T;
+        if (i <= m && psi[j]) atomicMax(&top, (int)i);
+      }
     }
   }
   __syncthreads();
@@ -156,15 +173,49 @@ rs_locator_kernel(const F f, const u64* __restrict__ Y, const uint8_t* __restric
   }
   __syncthreads();
   u64* o = out + b * ld;
-  for (u64 i = t; i < ld; i += T) {
-    u64 om = 0;
-    if (i < m)
-      for (u64 l = 0; l <= i; l++) om = f.add(om, f.mul(P[l], S[i - l]));
-    o[i] = i <= m ? P[i] : 0;
-    o[plane + i] = i < m ? f.mul((i + 1) % f.modulus(), P[i + 1]) : 0;
-    o[2 * plane + i] = om;
+  if constexpr (AT) {
+    // σ[i] = Ψ[L - i], σ'[i] = (i + 1)·Ψ[L - 1 - i], Ω̂[i] = Ω[L - 1 - i]; L ≤ m on a row that has not failed
+    const u64 L = fail ? 0 : deg;
+    for (u64 i = t; i < ld; i += T) {
+      u64 sg = 0, ds = 0, om = 0;
+      if (i <= L) sg = P[L - i];
+      if (i < L) {
+        const u64 e = L - 1 - i;
+        ds = f.mul((i + 1) % f.modulus(), P[e]);
+        for (u64 l = 0; l <= e; l++) om = f.add(om, f.mul(P[l], S[e - l]));
+      }
+      o[i] = sg;
+      o[plane + i] = ds;
+      o[2 * plane + i] = om;
+    }
+  } else {
+    for (u64 i = t; i < ld; i += T) {
+      u64 om = 0;
+      if (i < m)
+        for (u64 l = 0; l <= i; l++) om = f.add(om, f.mul(P[l], S[i - l]));
+      o[i] = i <= m ? P[i] : 0;
+      o[plane + i] = i < m ? f.mul((i + 1) % f.modulus(), P[i + 1]) : 0;
+      o[2 * plane + i] = om;
+    }
   }
   if (t == 0) rows[b] = RsRow{deg, eps, fail ? 1u : 0u, 0u};
+}
+
+// Y: the rows' scaled inverse transforms (batch × n); erased: batch × n bytes or null; winv = ω^-1.
+template <class F>
+__global__ void __launch_bounds__(RS_LOC_MAX_THREADS)
+rs_locator_kernel(const F f, const u64* __restrict__ Y, const uint8_t* __restrict__ erased, u64 n, u64 k, u64 winv,
+                  u64* __restrict__ out, u64 ld, u64 plane, RsRow* __restrict__ rows) {
+  rs_locator_body<F, false>(f, Y, 0, nullptr, erased, n, k, winv, out, ld, plane, rows);
+}
+
+// S: the rows' syndromes, m = n - k words at S + b·sld; xs: the n points; erased: batch × n bytes or null.
+template <class F>
+__global__ void __launch_bounds__(RS_LOC_MAX_THREADS)
+rs_locator_at_kernel(const F f, const u64* __restrict__ S, u64 sld, const u64* __restrict__ xs,
+                     const uint8_t* __restrict__ erased, u64 n, u64 k, u64* __restrict__ out, u64 ld, u64 plane,
+                     RsRow* __restrict__ rows) {
+  rs_locator_body<F, true>(f, S, sld, xs, erased, n, k, 0, out, ld, plane, rows);
 }
 
 // out[r·n + i] = scale · Σ_{j<len} a[r·lda + j] · ω^(±ij), r < rows: the literal transform of every row in one launch,
@@ -215,6 +266,38 @@ rs_correct_kernel(const F f, const u64* __restrict__ received, const u64* __rest
         atomicOr(&rows[b].fail, 1u);
       } else {
         const u64 x = f.mul(field_pow(f, w, i * (k - 1) % n), f.mul(neg_n, P[2 * plane + at]));
+        v = f.sub(v, f.mul(x, field_pow(f, dv, f.modulus() - 2)));
+      }
+    }
+    R[at] = v;
+  }
+}
+
+// out = received with its erased positions set to 0, over total words: the erased values are never read after this.
+__global__ void __launch_bounds__(RS_THREADS)
+rs_mask_kernel(const u64* __restrict__ received, const uint8_t* __restrict__ erased, u64 total, u64* __restrict__ out) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 at = (u64)blockIdx.x * blockDim.x + threadIdx.x; at < total; at += stride) out[at] = erased[at] ? 0 : received[at];
+}
+
+// rs_correct_kernel at any points: R = row - e over batch × n.  At a root x_i of σ (E: σ's values, plane words before
+// those of σ' and Ω̂), e_i = Ω̂(x_i)·M'(x_i) / σ'(x_i), W[i] = M'(x_i); counts the roots per row (at most L: deg σ = L,
+// and σ's roots among distinct points are distinct), and a root where σ' vanishes fails.
+template <class F>
+__global__ void __launch_bounds__(RS_THREADS)
+rs_forney_kernel(const F f, const u64* __restrict__ row, const u64* __restrict__ E, u64 plane, const u64* __restrict__ W, u64 n,
+                 RsRow* rows, u64* __restrict__ R) {
+  const u64 stride = (u64)gridDim.x * blockDim.x;
+  for (u64 at = (u64)blockIdx.x * blockDim.x + threadIdx.x; at < plane; at += stride) {
+    const u64 b = at / n, i = at - b * n;
+    u64 v = row[at];
+    if (!rows[b].fail && E[at] == 0) {
+      atomicAdd(&rows[b].roots, 1u);
+      const u64 dv = E[plane + at];
+      if (dv == 0) {
+        atomicOr(&rows[b].fail, 1u);
+      } else {
+        const u64 x = f.mul(E[2 * plane + at], W[i]);
         v = f.sub(v, f.mul(x, field_pow(f, dv, f.modulus() - 2)));
       }
     }
@@ -358,9 +441,130 @@ static int rs_decode_device(ronk_ctx* ctx, u64 p, u64 g, const u64* received, co
   });
 }
 
+// ---- decoding at any distinct points (ronk_rs_decode_at_u64) ---------------------------------------------------------
+// With m = n - k, M = Π (X - x_i), and I_b the interpolant of row b with its erasures zeroed:
+//   S_b(z) = Ĩ_b(z)·T(z) mod z^m, Ĩ_b[t] = I_b[n - 1 - t], T = 1 / (z^n·M(1/z)) mod z^m, the reversal of
+//   quo(X^(n+m-1), M); that is S_j = Σ_i r_i·x_i^j / M'(x_i), zero for a codeword (deg f·X^j ≤ n - 2);
+//   the locator above (AT) gives σ, σ', Ω̂ and L; one multieval of the 3·batch rows over xs, and M'(x_i) once;
+//   rs_forney corrects the roots of σ; C_b = interpolant of (row - e); rs_finish as for ronk_rs_decode_u64.
+// Every step is an existing batched entry point or kernel on its own path rule, and none picks its launches by the
+// batch save where those entry points do.
+
+// Checks that read no pointer's contents, in the documented order.
+static int rs_decode_at_args(ronk_ctx* ctx, u64 p, u64 g, const void* xs, const void* received, const void* erased, u64 n,
+                             u64 k, u32 batch, const void* msg, const void* status) {
+  if (!ctx || !xs || !received || !msg || !status) return set_err(ctx, RONK_EINVAL, "null argument");
+  RONK_TRY(validate_modulus(ctx, p));
+  if (g >= p) return set_err(ctx, RONK_EINVAL, "generator out of range");
+  if (n == 0 || k == 0 || k > n) return set_err(ctx, RONK_EINVAL, "need 0 < k <= n");
+  const u64 m = n - k;
+  if (m > kRsMaxParity) return set_err(ctx, RONK_EUNSUPPORTED, "n - k above kRsMaxParity = 8191");
+  if (n > kTreeMaxLeaves) return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^24 points");
+  if (3 * (u64)batch > 0xFFFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "3·batch rows above 2^32 - 1");
+  bool tree = false;
+  if (batch) {  // the path rules divide by the batch
+    RONK_TRY(interpolate_path(ctx, p, g, n, batch, &tree));
+    RONK_TRY(multieval_path(ctx, p, g, m + 1, 3 * batch, n, &tree));
+  }
+  if (m && ((u64)batch << log2_ceil(2 * m - 1)) > ((u64)1 << 32))
+    return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^32 words of syndrome products");
+  const size_t nx = n * 8, nr = (size_t)batch * n * 8, ne = (size_t)batch * n, nm = (size_t)batch * k * 8, ns = (size_t)batch * 4;
+  if (bytes_overlap(msg, nm, xs, nx) || bytes_overlap(msg, nm, received, nr) || bytes_overlap(msg, nm, erased, ne) ||
+      bytes_overlap(status, ns, xs, nx) || bytes_overlap(status, ns, received, nr) || bytes_overlap(status, ns, erased, ne) ||
+      bytes_overlap(msg, nm, status, ns))
+    return set_err(ctx, RONK_EINVAL, "output overlaps input");
+  return RONK_OK;
+}
+
+static int rs_decode_at_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, const u64* received, const uint8_t* erased, u64 n,
+                               u64 k, u32 batch, u64* msg, int32_t* status) {
+  RONK_TRY(rs_decode_at_args(ctx, p, g, xs, received, erased, n, k, batch, msg, status));
+  if (batch == 0) return RONK_OK;
+  const u64 m = n - k, plane = (u64)batch * n, lp = (u64)batch * (m + 1), ls = m ? 2 * m - 1 : 0;
+  // Z: the masked rows, then C | I: the interpolants, then row - e | M, M', M'(x_i) | X^(n+m-1), its quotient and
+  // remainder by M, T | Ĩ, S | σ, σ', Ω̂ | their values | rows
+  Frame fr(ctx);
+  u64* Z = nullptr;
+  RONK_TRY(fr.take(&Z, 2 * plane + 3 * n + 1 + (m ? 3 * (n + m) + m : 0) + (u64)batch * (m + ls) + 3 * lp + 3 * plane + 2 * (u64)batch));
+  u64* I = Z + plane;
+  u64* M = I + plane;
+  u64* Mp = M + n + 1;
+  u64* W = Mp + n;
+  u64* A = W + n;
+  u64* Q = A + (m ? n + m : 0);
+  u64* Rm = Q + (m ? n + m : 0);
+  u64* T = Rm + (m ? n + m : 0);
+  u64* IR = T + m;
+  u64* S = IR + (u64)batch * m;
+  u64* P = S + (u64)batch * ls;
+  u64* E = P + 3 * lp;
+  RsRow* rows = (RsRow*)(E + 3 * plane);
+  const u64* row = received;
+  if (erased) {
+    RONK_TRY(launch(ctx, "rs_mask", rs_mask_kernel, grid_for(ctx, plane, RS_THREADS), RS_THREADS, 0, false, received, erased,
+                    plane, Z));
+    row = Z;
+  }
+  // synchronises; RONK_EINVAL for a repeated point, before anything is written to msg or status
+  RONK_TRY(ronk_poly_interpolate_batch_u64(ctx, p, g, xs, row, n, batch, I));
+  RONK_TRY(ronk_poly_from_roots_u64(ctx, p, g, xs, n, M));
+  RONK_TRY(poly_deriv(ctx, p, M, n, Mp));
+  RONK_TRY(ronk_poly_multieval_batch_u64(ctx, p, g, Mp, n, 1, xs, n, W));
+  if (m) {
+    const u64 one = 1;  // X^(n+m-1) (pageable source: staged before cudaMemcpyAsync returns)
+    RONK_CUDA(ctx, cudaMemsetAsync(A, 0, (n + m - 1) * sizeof(u64), ctx->stream));
+    RONK_CUDA(ctx, cudaMemcpyAsync(A + n + m - 1, &one, sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
+    RONK_TRY(ronk_poly_divrem_u64(ctx, p, g, A, n + m, M, n + 1, Q, Rm));
+    RONK_TRY(reverse_words(ctx, "rs_reverse", Q, m - 1, m, T, m));
+    RONK_TRY(reverse_rows(ctx, I, n, n - 1, m, IR, m, m, batch));
+    RONK_TRY(ronk_poly_mul_batch_u64(ctx, p, g, IR, m, T, m, 1, batch, S));
+  }
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    using F = std::decay_t<decltype(f)>;
+    const u32 threads = (u32)std::min<u64>(RS_LOC_MAX_THREADS, std::max<u64>(32, ((m + 1 + RS_LOC_PER - 1) / RS_LOC_PER + 31) / 32 * 32));
+    RONK_TRY(ensure_smem_attr(ctx, rs_locator_at_kernel<F>, (int)((3 * kRsMaxParity + 2) * sizeof(u64))));
+    RONK_TRY(launch(ctx, "rs_locator_at", rs_locator_at_kernel<F>, batch, threads, (3 * m + 2) * sizeof(u64), false, f,
+                    (const u64*)S, ls, xs, erased, n, k, P, m + 1, lp, rows));
+    RONK_TRY(ronk_poly_multieval_batch_u64(ctx, p, g, P, m + 1, 3 * batch, xs, n, E));
+    RONK_TRY(launch(ctx, "rs_forney", rs_forney_kernel<F>, grid_for(ctx, plane, RS_THREADS), RS_THREADS, 0, false, f, row,
+                    (const u64*)E, plane, (const u64*)W, n, rows, I));
+    RONK_TRY(ronk_poly_interpolate_batch_u64(ctx, p, g, xs, I, n, batch, Z));
+    return launch(ctx, "rs_finish", rs_finish_kernel, dim3(batch, (unsigned)((k + RS_FIN_CHUNK - 1) / RS_FIN_CHUNK)), RS_THREADS,
+                  0, false, (const u64*)Z, n, k, (const RsRow*)rows, msg, status);
+  });
+}
+
 }  // namespace ronk
 
 using namespace ronk;
+
+extern "C" int ronk_rs_decode_at_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, const uint64_t* received,
+                                     const uint8_t* erased, uint64_t n, uint64_t k, uint32_t batch, uint64_t* msg,
+                                     int32_t* status) {
+  ronk::DeviceGuard _dg(ctx);
+  return rs_decode_at_device(ctx, p, g, (const u64*)xs, (const u64*)received, erased, n, k, batch, (u64*)msg, status);
+}
+
+extern "C" int ronk_rs_decode_at_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* xs, const uint64_t* received,
+                                          const uint8_t* erased, uint64_t n, uint64_t k, uint32_t batch, uint64_t* msg,
+                                          int32_t* status) {
+  ronk::DeviceGuard _dg(ctx);
+  RONK_TRY(rs_decode_at_args(ctx, p, g, xs, received, erased, n, k, batch, msg, status));  // before staging
+  for (u64 i = 0; i < n; i++)
+    if (xs[i] >= p) return set_err(ctx, RONK_EINVAL, "point out of range (x >= p)");
+  if (batch == 0) return RONK_OK;
+  Staged s[] = {{n * 8, xs},
+                {(size_t)batch * n * 8, received},
+                {erased ? (size_t)batch * n : 0, erased},
+                {(size_t)batch * k * 8, nullptr, msg},
+                {(size_t)batch * 4, nullptr, status}};
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
+  return stage_out(ctx,
+                   rs_decode_at_device(ctx, p, g, s[0].dev, s[1].dev, erased ? (const uint8_t*)s[2].dev : nullptr, n, k, batch,
+                                       s[3].dev, (int32_t*)s[4].dev),
+                   s);
+}
 
 extern "C" int ronk_rs_encode_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* msg, uint64_t k, uint64_t n,
                                   uint32_t batch, uint64_t* codeword) {

@@ -229,6 +229,25 @@ def rs_decode(ctx: Context, received, k: int, erased=None, batch: int = 1, p: in
     return msg, status
 
 
+def rs_decode_at(ctx: Context, xs, received, k: int, erased=None, batch: int = 1, p: int = GOLDILOCKS, g: int = 7):
+    """rs_decode for received words whose positions share any n distinct points xs (n words, canonical): returns new
+    tensors (messages, batch × k; status, int32 per row: the errors corrected, or -1 with a zero message for a row
+    outside the decoding radius).  erased: None or a uint8/bool tensor of batch × n, nonzero at erased positions, whose
+    received values are never read.  Synchronous; raises RonkPanic for a repeated point."""
+    import torch
+    _check_u64(xs); _check_u64(received)
+    n = xs.numel()
+    assert received.numel() == batch * n, "received is batch × len(xs)"
+    if erased is not None:
+        erased = erased.to(torch.uint8).contiguous()
+        assert erased.is_cuda and erased.numel() == received.numel()
+    msg = torch.empty(batch * k, dtype=torch.int64, device=received.device)
+    status = torch.empty(batch, dtype=torch.int32, device=received.device)
+    ctx.call("ronk_rs_decode_at_u64", p, g, _lib._ptr(xs), _lib._ptr(received), _lib._ptr(erased), n, k, batch,
+             _lib._ptr(msg), _lib._ptr(status))
+    return msg, status
+
+
 def field_binop(ctx: Context, op: str, a, b, p: int = GOLDILOCKS):
     import torch
     _check_u64(a); _check_u64(b)
