@@ -88,6 +88,8 @@ extern "C" {
   pub fn ronk_poly_divrem_u64_host(ctx: *mut ronk_ctx, p: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;
   /// `quotient_and_remainder` on device pointers; Newton iteration on the transforms when the divisor's top word is nonzero.
   pub fn ronk_poly_divrem_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, q: *mut u64, r: *mut u64) -> c_int;
+  pub fn ronk_poly_divrem_batch_u64(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, b_shared: c_int, batch: u32, q: *mut u64, r: *mut u64) -> c_int;
+  pub fn ronk_poly_divrem_batch_u64_host(ctx: *mut ronk_ctx, p: u64, g: u64, a: *const u64, da: usize, b: *const u64, db: usize, b_shared: c_int, batch: u32, q: *mut u64, r: *mut u64) -> c_int;
   /// Lagrange interpolation = `Message::decode` on the first K coordinates (src/codes/reed_solomon.rs:55-107); host pointers.
   pub fn ronk_poly_interpolate_u64_host(ctx: *mut ronk_ctx, p: u64, xs: *const u64, ys: *const u64, k: usize, out: *mut u64) -> c_int;
   /// Π (X - xs[i]) on device pointers, k + 1 coefficients; a subproduct tree on the transforms above the crossover.

@@ -322,6 +322,38 @@ int ronk_poly_divrem_u64_host(ronk_ctx *ctx, uint64_t p, const uint64_t *a, size
  * iteration on the transforms (a fixed number of transforms instead of O(da·(da - db)) sequential steps).  g == 0,
  * or a prime with too few 2-power roots of unity (p = 101, 17, 127), keeps the literal kernel.  Residues canonical. */
 int ronk_poly_divrem_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db, uint64_t *q, uint64_t *r);
+/* `batch` divisions at once: row y of q and r is exactly what ronk_poly_divrem_u64(p, g, a[y], b_shared ? b : b[y]) gives,
+ * on every prime and path, the reference's quirks for a zero top word included.  Rows are contiguous, in the order of
+ * ronk_poly_mul_batch_u64: a is batch × da, b is batch × db (db words when b_shared), q and r are batch × da each.
+ * - Errors, in this order: (1) without reading a pointer: RONK_EINVAL for a null pointer (when batch·da > 0), an invalid
+ *   modulus or g >= p; RONK_EUNSUPPORTED for da or db above 0x7FFFFFF0, batch·da or batch·db above 2^40 words, and, where
+ *   the path rule below puts rows with nonzero top words on Newton iteration, batch × the plan's larger transform above
+ *   2^32 words; (2) RONK_EINVAL for a q or r that overlaps a, b or the other output; (3) the divisors' top words are read
+ *   back; (4) RONK_EINVAL where any row panics in the reference, as the single-row entry does on it.  After (1) and (2)
+ *   nothing is written; after (4) the words of q and r are unspecified.  batch == 0 or da == 0 does nothing.
+ * - Batch 1 is ronk_poly_divrem_u64 itself: same words, same launches.  From batch 2, with L = da − db + 1, one path for
+ *   the whole call:
+ *   any top word 0 (any row, or the shared b; db == 0): every row on the literal kernel, one CTA per row.  A row with a
+ *     nonzero top word gets its Euclidean words from that kernel too, so the batch is never split;
+ *   da < db: q = 0 and r = a (one memset, one copy);
+ *   db == 2: the scan of ronk_poly_div_linear_u64 over every row (z = −b0/b1 and b1^-1 per row: on the host for a shared
+ *     divisor, in one launch otherwise); r[0] = a(z) and the rest of each r is 0.  Scratch 2·batch·⌈da/4096⌉ + 2·batch words;
+ *   Newton iteration where its transforms fit (as ronk_poly_divrem_u64) and the measured rule prefers it (DESIGN.md §5):
+ *     one inverse of rev(b) (shared) or one batched inversion of every row's, then the quotient and the remainder's low
+ *     words as batched cyclic products.  Scratch rows·(L + min(db, L) + N) + batch·N words plus the transforms' workspace
+ *     (batch·N words past 2^15 points) and 8·256 bytes, N = the larger of the plan's two transforms, rows = 1 when b_shared
+ *     else batch.  Taken before the first launch that writes q or r;
+ *   otherwise the literal kernel over every row.
+ *   RONK_DIVREM_BATCH_PATH forces literal (1) or Newton wherever it fits (2) from batch 2 (INTEGRATION.md).
+ * - Synchronous: the top words are read back once (one copy of a shared divisor's top, or b[0..2) when db == 2; one scan
+ *   launch over per-row divisors), the literal path reads its panic flag.  The launch sequence from batch 2 depends on the
+ *   batch only where ronk_ntt_u64 picks its kernels by batch at 2^16 points.
+ * - The _host twin makes every check of (1) before it stages anything, stages in and out and synchronises.  Residues
+ *   canonical; 8-byte alignment; no word past a[batch·da), b[batch·db) (b[db) when shared), q or r[batch·da) is touched. */
+int ronk_poly_divrem_batch_u64(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b, size_t db,
+                               int b_shared, uint32_t batch, uint64_t *q, uint64_t *r);
+int ronk_poly_divrem_batch_u64_host(ronk_ctx *ctx, uint64_t p, uint64_t g, const uint64_t *a, size_t da, const uint64_t *b,
+                                    size_t db, int b_shared, uint32_t batch, uint64_t *q, uint64_t *r);
 /* Division by a linear factor b0 + b1*x — the divisor kzg::open builds (src/kzg/setup.rs:72-75,
  * [-z, 1]) fed to Polynomial::div (src/polynomial/mod.rs:170-225, arithmetic.rs:121-146) — as a
  * device-wide scan.  Device pointers: a (d terms), q (d terms, q[d-1] = 0 like the reference's

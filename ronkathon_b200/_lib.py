@@ -78,6 +78,8 @@ SIGNATURES = {
     "ronk_poly_lagrange_open_u64_host": (i32, [vp, u64, u64, vp, u64, u32, u64, u64, vp, vp]),
     "ronk_poly_divrem_u64_host": (i32, [vp, u64, vp, sz, vp, sz, vp, vp]),
     "ronk_poly_divrem_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, vp, vp]),
+    "ronk_poly_divrem_batch_u64": (i32, [vp, u64, u64, vp, sz, vp, sz, i32, u32, vp, vp]),
+    "ronk_poly_divrem_batch_u64_host": (i32, [vp, u64, u64, vp, sz, vp, sz, i32, u32, vp, vp]),
     "ronk_poly_div_linear_u64": (i32, [vp, u64, vp, sz, u64, u64, vp, vp]),
     "ronk_poly_interpolate_u64_host": (i32, [vp, u64, vp, vp, sz, vp]),
     "ronk_poly_from_roots_u64": (i32, [vp, u64, u64, vp, sz, vp]),

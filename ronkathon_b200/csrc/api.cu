@@ -66,6 +66,7 @@ int ronk_ctx_create(ronk_ctx** out, int device, void* stream) {
   const char* crt_min = getenv("RONK_CRT_MUL_MIN");
   ctx->tune.crt_mul_min = crt_min ? strtoll(crt_min, nullptr, 10) : -1;
   ctx->tune.poly_batch_path = env_int("RONK_POLY_BATCH_PATH", 0);
+  ctx->tune.divrem_batch_path = env_int("RONK_DIVREM_BATCH_PATH", 0);
   ctx->stream = (cudaStream_t)stream;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return RONK_ECUDA; }

@@ -108,10 +108,10 @@ __global__ void lagrange_eval_kernel(const F f, const u64* c, const u64* nodes, 
   if (t == 0) out[0] = f.mul(lred[0], red[0]);
 }
 
-// quotient_and_remainder (mod.rs:170-225).  Single CTA; q and r have da terms.
+// quotient_and_remainder (mod.rs:170-225) of one row by the whole CTA; q and r have da terms.
 // flag: 1 = all-zero divisor / non-invertible, 2 = index out of range (the reference panics).
 template <class F>
-__global__ void poly_divrem_kernel(const F f, const u64* a, u32 da, const u64* b, u32 db, u64* q, u64* r, int* flag) {
+__device__ __forceinline__ void divrem_row(const F& f, const u64* a, u32 da, const u64* b, u32 db, u64* q, u64* r, int* flag) {
   __shared__ u32 s_deg, s_ok;
   __shared__ u64 s_s;
   const u32 t = threadIdx.x, nt = blockDim.x;
@@ -160,6 +160,23 @@ __global__ void poly_divrem_kernel(const F f, const u64* a, u32 da, const u64* b
   }
 }
 
+// Single CTA, one row.
+template <class F>
+__global__ void poly_divrem_kernel(const F f, const u64* a, u32 da, const u64* b, u32 db, u64* q, u64* r, int* flag) {
+  divrem_row(f, a, da, b, db, q, r, flag);
+}
+
+// `batch` rows (a, q, r: batch × da; b: rows b_stride apart, 0 for one shared divisor), one CTA per row, stepping by
+// gridDim.y.  The barrier keeps a fast thread's next row from resetting the shared scalars a slow one still reads.
+template <class F>
+__global__ void poly_divrem_rows_kernel(const F f, const u64* a, u32 da, const u64* b, u32 db, u64 b_stride, u32 batch, u64* q,
+                                        u64* r, int* flag) {
+  for (u64 row = blockIdx.y; row < batch; row += gridDim.y) {
+    divrem_row(f, a + row * da, da, b + row * b_stride, db, q + row * da, r + row * da, flag);
+    __syncthreads();
+  }
+}
+
 
 // ---- division by a linear factor (b0 + b1·x), §8f row 1 ------------------------------------------
 // quotient_and_remainder (mod.rs:170-225) specialised to the divisor kzg::open builds
@@ -179,9 +196,8 @@ RONK_DEV u64 pow2k_tw(const F& f, u64 x_tw, int k) {  // x^(2^k), twiddle form i
 }
 
 template <class F, bool APPLY>
-__global__ void __launch_bounds__(DL_THR)
-div_linear_kernel(const F f, const u64* __restrict__ a, u64 d, u64 z, const u64* __restrict__ carry, u64* __restrict__ S,
-                  u64 scale, u64* __restrict__ q, u64* __restrict__ rem) {
+__device__ __forceinline__ void div_linear_chunk(const F& f, const u64* __restrict__ a, u64 d, u64 z, const u64* __restrict__ carry,
+                                                 u64* __restrict__ S, u64 scale, u64* __restrict__ q, u64* __restrict__ rem) {
   __shared__ u64 tile[DL_CHUNK + DL_CHUNK / 16];
   __shared__ u64 v[DL_THR + 1];
   const u32 tid = threadIdx.x;
@@ -230,11 +246,17 @@ div_linear_kernel(const F f, const u64* __restrict__ a, u64 d, u64 z, const u64*
   if (c0 + DL_CHUNK >= d && c0 < d && tid == 0) q[d - 1] = 0ULL;
 }
 
+template <class F, bool APPLY>
+__global__ void __launch_bounds__(DL_THR)
+div_linear_kernel(const F f, const u64* __restrict__ a, u64 d, u64 z, const u64* __restrict__ carry, u64* __restrict__ S,
+                  u64 scale, u64* __restrict__ q, u64* __restrict__ rem) {
+  div_linear_chunk<F, APPLY>(f, a, d, z, carry, S, scale, q, rem);
+}
+
 // carry[c] = Σ_{c' > c} S_{c'} Z^{c'-c-1}, Z = z^4096.  One CTA: every thread owns a contiguous block of
 // chunks (local Horner), thread 0 chains the ≤ 1024 block values, then every thread replays its block.
 template <class F>
-__global__ void __launch_bounds__(1024)
-div_linear_carry_kernel(const F f, const u64* __restrict__ S, u32 nchunks, u64 z, u64* __restrict__ carry) {
+__device__ __forceinline__ void div_linear_carries(const F& f, const u64* __restrict__ S, u32 nchunks, u64 z, u64* __restrict__ carry) {
   __shared__ u64 L[1024];
   __shared__ u64 G[1025];
   const u32 t = threadIdx.x;
@@ -266,6 +288,38 @@ div_linear_carry_kernel(const F f, const u64* __restrict__ S, u32 nchunks, u64 z
   for (u32 c = hi; c-- > lo;) {
     carry[c] = run;
     run = f.add(S[c], f.mul_tw(run, Z));
+  }
+}
+
+template <class F>
+__global__ void __launch_bounds__(1024)
+div_linear_carry_kernel(const F f, const u64* __restrict__ S, u32 nchunks, u64 z, u64* __restrict__ carry) {
+  div_linear_carries(f, S, nchunks, z, carry);
+}
+
+// The three kernels above over `batch` rows of d words (a, q, rem: rows d apart; S, carry: rows nchunks apart), row y
+// stepping by gridDim.y, dividing by its own linear factor: zs[y·zstride] = b1^-1 and zs[y·zstride + 1] = z (zstride 0
+// for one shared divisor).  rem[y·d] = a_y(z).  The barrier keeps one row's shared-memory reads ahead of the next row's
+// writes.
+template <class F, bool APPLY>
+__global__ void __launch_bounds__(DL_THR)
+div_linear_rows_kernel(const F f, const u64* __restrict__ a, u64 d, const u64* __restrict__ zs, u32 zstride, u32 batch,
+                       const u64* __restrict__ carry, u64* __restrict__ S, u64 nchunks, u64* __restrict__ q, u64* __restrict__ rem) {
+  for (u64 y = blockIdx.y; y < batch; y += gridDim.y) {
+    const u64 scale = zs[y * zstride], z = zs[y * zstride + 1];
+    div_linear_chunk<F, APPLY>(f, a + y * d, d, z, APPLY ? carry + y * nchunks : nullptr, APPLY ? nullptr : S + y * nchunks,
+                               scale, APPLY ? q + y * d : nullptr, APPLY ? rem + y * d : nullptr);
+    __syncthreads();
+  }
+}
+
+template <class F>
+__global__ void __launch_bounds__(1024)
+div_linear_rows_carry_kernel(const F f, const u64* __restrict__ S, u32 nchunks, const u64* __restrict__ zs, u32 zstride, u32 batch,
+                             u64* __restrict__ carry) {
+  for (u64 y = blockIdx.y; y < batch; y += gridDim.y) {
+    div_linear_carries(f, S + y * nchunks, nchunks, zs[y * zstride + 1], carry + y * nchunks);
+    __syncthreads();
   }
 }
 
@@ -333,6 +387,128 @@ static int divrem_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, c
     int v = 0;
     RONK_TRY(read_flag(ctx, &v));  // synchronises the stream
     if (v) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on this divisor");
+    return RONK_OK;
+  }
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return RONK_OK;
+}
+
+// The single-row entries are batch = 1 without `reserve`; the batched ones take all the call's scratch before the first
+// launch (reserve), so that what follows fits the blocks that take leaves.
+static int reserve_scratch(ronk_ctx* ctx, size_t words) {
+  Frame fr(ctx);
+  u64* all = nullptr;
+  return fr.take(&all, words);
+}
+
+// ---- batches of divisions (ronk_poly_divrem_batch_u64) -------------------------------------------------------------
+// flag = 1 when any of the batch rows of b (db words each, db ≥ 1) has a zero top word
+__global__ void divrem_top_scan_kernel(const u64* __restrict__ b, size_t db, u32 batch, int* flag) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t y = (size_t)blockIdx.x * blockDim.x + threadIdx.x; y < batch; y += stride)
+    if (b[y * db + db - 1] == 0) atomicExch(flag, 1);
+}
+
+enum DivremBatchPath { DB_COPY, DB_LINEAR, DB_NEWTON, DB_LITERAL };
+
+constexpr u64 kDivremBatchMaxWords = (u64)1 << 40, kDivremBatchMaxTransformWords = (u64)1 << 32;
+
+// Newton iteration or the literal kernel, from batch 2, for rows whose top words are nonzero (da ≥ db, db != 2).  The
+// literal kernel runs one CTA per row, sm_count·8 rows at a time, each about L sequential steps over the dividend's
+// shrinking top; Newton costs at least about 0.3 ms (its launches and transforms) and won wherever the literal estimate
+// passed that.  tools/divrem_batch_timing.py on an H100 80GB HBM3 at 700 W (DESIGN.md §5), Goldilocks: the literal
+// kernel took about 0.09 ms per wave of rows plus 1 µs per 2000 words of L·(da + db) (64 × 17: 0.10 ms, 256 × 17:
+// 0.21, 1024 × 17: 1.02, 4096 × 2049: 8.5), Newton 0.22 … 0.47 ms up to da = 1024 at up to 4096 rows.  On BabyBear
+// (the Montgomery policy) both cost 10–40 % more and cross at the same shapes, so one rule serves both policies.
+static bool divrem_batch_newton(const ronk_ctx* ctx, u64 p, u64 g, size_t da, size_t db, u32 batch) {
+  if (!divrem_newton_fits(p, g, da, db)) return false;
+  if (ctx->tune.divrem_batch_path) return ctx->tune.divrem_batch_path == 2;
+  const u64 L = da - db + 1, slots = (u64)ctx->sm_count * 8, waves = (batch + slots - 1) / slots;
+  return waves * (90 + L * (da + db) / 2000) >= 300;  // µs; da, db ≤ 2^26 where Newton fits
+}
+
+// The checks that read no pointer, in the header's order, and the path of rows whose top words are nonzero.
+static int divrem_batch_args(ronk_ctx* ctx, u64 p, u64 g, bool null_arg, size_t da, size_t db, bool b_shared, u32 batch,
+                             DivremBatchPath* path) {
+  if (!ctx || null_arg) return set_err(ctx, RONK_EINVAL, "null argument");
+  RONK_TRY(validate_modulus(ctx, p));
+  if (g >= p) return set_err(ctx, RONK_EINVAL, "generator out of range");
+  if (da > 0x7FFFFFF0ULL || db > 0x7FFFFFF0ULL) return set_err(ctx, RONK_EUNSUPPORTED, "polynomial too long");
+  if ((u64)batch * da > kDivremBatchMaxWords || (b_shared ? db : (u64)batch * db) > kDivremBatchMaxWords)
+    return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^40 words in a, b, q or r");
+  *path = db == 0 ? DB_LITERAL : da < db ? DB_COPY : db == 2 ? DB_LINEAR
+          : batch > 1 && divrem_batch_newton(ctx, p, g, da, db, batch) ? DB_NEWTON : DB_LITERAL;
+  if (*path == DB_NEWTON && divrem_newton_rows_transform_words(da, db, batch) > kDivremBatchMaxTransformWords)
+    return set_err(ctx, RONK_EUNSUPPORTED, "more than 2^32 words of batched transforms");
+  return RONK_OK;
+}
+
+static int divrem_batch_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, bool b_shared,
+                               u32 batch, u64* q, u64* r) {
+  const bool empty = batch == 0 || da == 0;
+  DivremBatchPath path;
+  RONK_TRY(divrem_batch_args(ctx, p, g, !empty && (!a || !q || !r || (db && !b)), da, db, b_shared, batch, &path));
+  if (empty) return RONK_OK;
+  const size_t na = (size_t)batch * da, nb = b_shared ? db : (size_t)batch * db;
+  if (overlaps(q, na, a, na) || overlaps(q, na, b, nb) || overlaps(r, na, a, na) || overlaps(r, na, b, nb) || overlaps(q, na, r, na))
+    return set_err(ctx, RONK_EINVAL, "q and r may not alias a, b or each other");
+  if (batch == 1) return divrem_device(ctx, p, g, a, da, b, db, q, r);
+  // the divisors' top words (and a shared linear divisor's b[0]), once for all rows
+  u64 lo_top[2] = {0, 0};
+  if (db && b_shared) {
+    const size_t w = db == 2 ? 2 : 1;
+    RONK_CUDA(ctx, cudaMemcpyAsync(lo_top + 2 - w, b + db - w, w * sizeof(u64), cudaMemcpyDeviceToHost, ctx->stream));
+    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (lo_top[1] == 0) path = DB_LITERAL;
+  } else if (db) {
+    RONK_TRY(reset_flag(ctx));
+    RONK_TRY(launch(ctx, "divrem_top_scan", divrem_top_scan_kernel, grid_for(ctx, batch, 256), 256, 0, false, b, db, batch,
+                    ctx->d_flag));
+    int zero = 0;
+    RONK_TRY(read_flag(ctx, &zero));
+    if (zero) path = DB_LITERAL;
+  }
+  const size_t bs = b_shared ? 0 : db;
+  if (path == DB_COPY) {  // the reference's loop never runs
+    RONK_CUDA(ctx, cudaMemsetAsync(q, 0, na * sizeof(u64), ctx->stream));
+    RONK_CUDA(ctx, cudaMemcpyAsync(r, a, na * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
+  } else if (path == DB_LINEAR) {
+    const size_t nchunks = (da + DL_CHUNK - 1) / DL_CHUNK;
+    Frame fr(ctx);
+    u64* S = nullptr;
+    RONK_TRY(fr.take(&S, 2 * (size_t)batch * nchunks + (b_shared ? 2 : 2 * (size_t)batch)));
+    u64* carry = S + (size_t)batch * nchunks;
+    u64* zs = carry + (size_t)batch * nchunks;  // [b1^-1, z] per row, or once
+    if (b_shared) {  // pageable source: staged before cudaMemcpyAsync returns
+      const u64 inv = h_powmod(lo_top[1], p - 2, p), z_inv[2] = {inv, h_mulmod(lo_top[0] ? p - lo_top[0] : 0, inv, p)};
+      RONK_CUDA(ctx, cudaMemcpyAsync(zs, z_inv, sizeof(z_inv), cudaMemcpyHostToDevice, ctx->stream));
+    } else {
+      RONK_TRY(divrem_top_inverses(ctx, p, b, db, batch, zs));
+    }
+    RONK_CUDA(ctx, cudaMemsetAsync(r, 0, na * sizeof(u64), ctx->stream));
+    const u32 zstride = b_shared ? 0 : 2;
+    RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+      using F = std::decay_t<decltype(f)>;
+      const dim3 grid((u32)nchunks, grid_rows(ctx, batch, nchunks));
+      RONK_TRY(launch(ctx, "div_linear_fold", div_linear_rows_kernel<F, false>, grid, DL_THR, 0, false, f, a, (u64)da,
+                      (const u64*)zs, zstride, batch, (const u64*)nullptr, S, (u64)nchunks, (u64*)nullptr, (u64*)nullptr));
+      RONK_TRY(launch(ctx, "div_linear_carry", div_linear_rows_carry_kernel<F>, dim3(1, grid_rows(ctx, batch, 1)), 1024, 0, false, f,
+                      (const u64*)S, (u32)nchunks, (const u64*)zs, zstride, batch, carry));
+      return launch(ctx, "div_linear_apply", div_linear_rows_kernel<F, true>, grid, DL_THR, 0, false, f, a, (u64)da, (const u64*)zs,
+                    zstride, batch, (const u64*)carry, (u64*)nullptr, (u64)nchunks, q, r);
+    }));
+  } else if (path == DB_NEWTON) {
+    RONK_TRY(reserve_scratch(ctx, divrem_newton_rows_scratch(da, db, b_shared, batch)));
+    RONK_TRY(divrem_newton_rows(ctx, p, g, a, da, b, db, b_shared, batch, lo_top[1], q, r));
+  } else {  // the literal long division, also for every row when any top word is zero
+    RONK_TRY(reset_flag(ctx));
+    RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+      return launch(ctx, "poly_divrem_rows", poly_divrem_rows_kernel<std::decay_t<decltype(f)>>, dim3(1, grid_rows(ctx, batch, 1)),
+                    256, 0, false, f, a, (u32)da, b, (u32)db, (u64)bs, batch, q, r, ctx->d_flag);
+    }));
+    int v = 0;
+    RONK_TRY(read_flag(ctx, &v));  // synchronises the stream
+    if (v) return set_err(ctx, RONK_EINVAL, "polynomial division: the reference would panic on a divisor of this batch");
     return RONK_OK;
   }
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -578,14 +754,6 @@ static int from_roots_device(ronk_ctx* ctx, u64 p, u64 g, const u64* xs, size_t 
 // the root's 2^⌈log2(2d - 1)⌉), as ronk_poly_mul_batch_u64's batched transforms; batch·⌈k/256⌉·8·k words of the literal
 // interpolation's per-warp partial sums.
 constexpr u64 kTreeBatchMaxWords = (u64)1 << 32;
-
-// The single-row entries are batch = 1 without `reserve`; the batched ones take all the call's scratch before the first
-// launch (reserve), so that what follows fits the blocks that take leaves.
-static int reserve_scratch(ronk_ctx* ctx, size_t words) {
-  Frame fr(ctx);
-  u64* all = nullptr;
-  return fr.take(&all, words);
-}
 
 // The path of a non-empty call and the checks that go with it, which read no pointer, so that the _host twins make them
 // before they stage anything: *tree, or RONK_EUNSUPPORTED past the envelope.
@@ -841,6 +1009,27 @@ int ronk_poly_interpolate_batch_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, 
   Frame fr(ctx);
   RONK_TRY(stage_in(fr, s));
   return stage_out(ctx, interpolate_device(ctx, p, g, s[0].dev, s[1].dev, k, batch, s[2].dev, true), s);
+}
+
+int ronk_poly_divrem_batch_u64(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* a, size_t da, const uint64_t* b, size_t db,
+                               int b_shared, uint32_t batch, uint64_t* q, uint64_t* r) {
+  ronk::DeviceGuard _dg(ctx);
+  return divrem_batch_device(ctx, p, g, (const u64*)a, da, (const u64*)b, db, b_shared != 0, batch, (u64*)q, (u64*)r);
+}
+
+// Host pointers: every check that reads no pointer comes first, so that nothing is staged for an empty or refused call.
+int ronk_poly_divrem_batch_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, const uint64_t* a, size_t da, const uint64_t* b,
+                                    size_t db, int b_shared, uint32_t batch, uint64_t* q, uint64_t* r) {
+  ronk::DeviceGuard _dg(ctx);
+  const bool empty = batch == 0 || da == 0;
+  DivremBatchPath path;
+  RONK_TRY(divrem_batch_args(ctx, p, g, !empty && (!a || !q || !r || (db && !b)), da, db, b_shared != 0, batch, &path));
+  if (empty) return RONK_OK;
+  const size_t na = (size_t)batch * da, nb = b_shared ? db : (size_t)batch * db;
+  Staged s[] = {{na * 8, a}, {nb * 8, b}, {na * 8, nullptr, q}, {na * 8, nullptr, r}};
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
+  return stage_out(ctx, divrem_batch_device(ctx, p, g, s[0].dev, da, s[1].dev, db, b_shared != 0, batch, s[2].dev, s[3].dev), s);
 }
 
 // ronk_poly_divrem_u64 with g = 0 (no Newton path) on staged copies of a and b.  Its checks up to da == 0 run before

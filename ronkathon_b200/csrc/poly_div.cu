@@ -151,4 +151,188 @@ int divrem_newton_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, c
   });
 }
 
+// ---- batches of rows (ronk_poly_divrem_batch_u64, poly.cu) ---------------------------------------------------------
+// out[y·os] = top_y^-1 and, with_z, out[y·os + 1] = z_y = -b_y[0]·top_y^-1, top_y = b_y[db - 1] != 0 (rows db apart)
+template <class F>
+__global__ void divrem_top_inv_kernel(const F f, const u64* __restrict__ b, size_t db, u32 batch, u64* __restrict__ out, size_t os,
+                                      bool with_z) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t y = (size_t)blockIdx.x * blockDim.x + threadIdx.x; y < batch; y += stride) {
+    const u64 inv = field_pow(f, b[y * db + db - 1], f.modulus() - 2);
+    out[y * os] = inv;
+    if (with_z) out[y * os + 1] = f.mul(f.sub(0, b[y * db]), inv);
+  }
+}
+
+// dst[y·n + k] = Σ_j src[y·ss + k + j·n] over k + j·n < len, k < n (n = 2^log_n): the rows mod x^n - 1, zero-padded;
+// total = rows·n
+template <class F>
+__global__ void divrem_rows_fold_kernel(const F f, const u64* __restrict__ src, size_t ss, size_t len, u32 log_n, u64 total,
+                                        u64* __restrict__ dst) {
+  const u64 step = (u64)gridDim.x * blockDim.x, n = (u64)1 << log_n;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += step) {
+    const u64* row = src + (i >> log_n) * ss;
+    u64 acc = 0;
+    for (u64 k = i & (n - 1); k < len; k += n) acc = f.add(acc, row[k]);
+    dst[i] = acc;
+  }
+}
+
+// dst[y·ds + k] = src[y·ss + k], k < n; total = rows·n
+__global__ void divrem_rows_copy_kernel(const u64* __restrict__ src, size_t ss, size_t n, u64* __restrict__ dst, size_t ds,
+                                        u64 total) {
+  const u64 step = (u64)gridDim.x * blockDim.x;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += step) {
+    const u64 y = i / n, k = i - y * n;
+    dst[y * ds + k] = src[y * ss + k];
+  }
+}
+
+// r[y·da + k] = k < rw ? Σ_j a[y·da + k + j·na] - P[y·np + k] : 0 (j over k + j·na < da), total = rows·da: the remainder
+// from the low words of b·q, with the dividend taken mod x^na - 1 (na = da: not folded)
+template <class F>
+__global__ void divrem_rows_rem_kernel(const F f, const u64* __restrict__ a, size_t da, size_t na, const u64* __restrict__ P,
+                                       size_t np, size_t rw, u64 total, u64* __restrict__ r) {
+  const u64 step = (u64)gridDim.x * blockDim.x;
+  for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += step) {
+    const u64 y = i / da, k = i - y * da;
+    if (k >= rw) {
+      r[i] = 0;
+      continue;
+    }
+    u64 acc = 0;
+    for (u64 j = k; j < da; j += na) acc = f.add(acc, a[y * da + j]);
+    r[i] = f.sub(acc, P[y * np + k]);
+  }
+}
+
+template <class F>
+static int rows_fold(ronk_ctx* ctx, const F& f, const u64* src, size_t ss, size_t len, u32 log_n, u32 rows, u64* dst) {
+  const u64 total = (u64)rows << log_n;
+  return launch(ctx, "divrem_rows_fold", divrem_rows_fold_kernel<F>, grid_for(ctx, total, 256), 256, 0, false, f, src, ss, len,
+                log_n, total, dst);
+}
+
+// The cyclic products of X's batch rows (2^log_n words each, zero-padded, untransformed) by B's rows (one shared row, or
+// batch): returns the buffer that holds them.
+static u64* rows_product(ronk_ctx* ctx, u64 p, u64 g, u64* X, u64* B, u32 log_n, u32 batch, bool shared, int* rc) {
+  if (shared) {
+    if ((*rc = ntt_device(ctx, p, g, B, nullptr, log_n, 1, 0)) != RONK_OK) return nullptr;
+    if ((*rc = ntt_device_shared_mul(ctx, p, g, X, X, B, log_n, batch)) != RONK_OK) return nullptr;
+    *rc = ntt_device(ctx, p, g, X, nullptr, log_n, batch, 1);
+    return X;
+  }
+  if ((*rc = ntt_device(ctx, p, g, X, nullptr, log_n, batch, 0)) != RONK_OK) return nullptr;
+  if ((*rc = ntt_device(ctx, p, g, B, X, log_n, batch, 0)) != RONK_OK) return nullptr;  // B̂ ⊙ X̂ fused into the last pass
+  *rc = ntt_device(ctx, p, g, B, nullptr, log_n, batch, 1);
+  return B;
+}
+
+// The regions of the batched plan: G (the inverses, rows L apart) | HR (rev(b) cut to hl words) | X (batch rows of nx) |
+// B (the other operand's rows of nx: one shared row, or batch).
+struct DivremRows {
+  size_t L, hl, rw, nq, nr, nx;
+  u32 lq, lr;
+  u32 rows_b;
+};
+
+static DivremRows divrem_rows_plan(size_t da, size_t db, bool b_shared, u32 batch) {
+  DivremRows d;
+  d.L = da - db + 1;
+  d.hl = std::min(db, d.L);
+  d.rw = db - 1;
+  divrem_newton_sizes(da, db, &d.lq, &d.lr);
+  d.nq = (size_t)1 << d.lq;
+  d.nr = (size_t)1 << d.lr;
+  d.nx = std::max(d.nq, d.nr);
+  d.rows_b = b_shared ? 1 : batch;
+  return d;
+}
+
+u64 divrem_newton_rows_transform_words(size_t da, size_t db, u32 batch) {
+  u32 lq, lr;
+  divrem_newton_sizes(da, db, &lq, &lr);
+  return (u64)batch << std::max(lq, lr);
+}
+
+size_t divrem_newton_rows_scratch(size_t da, size_t db, bool b_shared, u32 batch) {
+  const DivremRows d = divrem_rows_plan(da, db, b_shared, batch);
+  const size_t words = d.rows_b * (d.L + d.hl + d.nx) + (size_t)batch * d.nx;
+  return words + ntt_workspace_words(std::max(d.lq, d.lr), batch) + 8 * Frame::kAlign / 8;
+}
+
+template <class F>
+static int divrem_newton_rows_with_field(ronk_ctx* ctx, const F& f, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db,
+                                         bool b_shared, u32 batch, u64 top, u64* q, u64* r) {
+  const DivremRows d = divrem_rows_plan(da, db, b_shared, batch);
+  const size_t L = d.L, hl = d.hl, rw = d.rw, nq = d.nq, nr = d.nr;
+  Frame fr(ctx);
+  u64 *G = nullptr, *HR = nullptr, *X = nullptr, *B = nullptr;
+  RONK_TRY(fr.take(&G, d.rows_b * L));
+  RONK_TRY(fr.take(&HR, d.rows_b * hl));
+  RONK_TRY(fr.take(&X, (size_t)batch * d.nx));
+  RONK_TRY(fr.take(&B, d.rows_b * d.nx));
+  // (1) the inverses of rev(b) mod x^L
+  RONK_TRY(reverse_rows(ctx, b, db, db - 1, hl, HR, hl, hl, d.rows_b));
+  if (b_shared) {
+    RONK_TRY(newton_inverse(ctx, f, p, g, HR, hl, L, h_powmod(top, p - 2, p), G, X, X + nq));  // batch ≥ 2: 2·nq ≤ batch·nx
+  } else {  // the doubling steps of newton_inverse on batched transforms of every row
+    RONK_TRY(launch(ctx, "divrem_top_inv", divrem_top_inv_kernel<F>, grid_for(ctx, batch, 256), 256, 0, false, f, b, db, batch, G,
+                    L, false));
+    for (size_t t = 1; t < L; t *= 2) {
+      const size_t m = std::min(2 * t, L);
+      const u32 ln = log2_ceil(4 * t);
+      const u64 total = (u64)batch << ln;
+      const int grid = grid_for(ctx, total, PAD_THREADS);
+      RONK_TRY(launch(ctx, "poly_rows_pad", poly_rows_pad_kernel, grid, PAD_THREADS, 0, false, HR, (u32)std::min(hl, m), (u64)hl, ln,
+                      total, B));
+      RONK_TRY(launch(ctx, "poly_rows_pad", poly_rows_pad_kernel, grid, PAD_THREADS, 0, false, G, (u32)t, (u64)L, ln, total, X));
+      RONK_TRY(ntt_device(ctx, p, g, B, nullptr, ln, batch, 0));
+      RONK_TRY(ntt_device(ctx, p, g, X, nullptr, ln, batch, 0));
+      RONK_TRY(launch(ctx, "divrem_newton_step", divrem_newton_step_kernel<F>, grid_for(ctx, total, 256), 256, 0, false, f, X,
+                      (const u64*)B, (size_t)total));
+      RONK_TRY(ntt_device(ctx, p, g, X, nullptr, ln, batch, 1));
+      const u64 copied = (u64)batch * m;
+      RONK_TRY(launch(ctx, "divrem_rows_copy", divrem_rows_copy_kernel, grid_for(ctx, copied, 256), 256, 0, false, (const u64*)X,
+                      (size_t)1 << ln, m, G, L, copied));
+    }
+  }
+  // (2) rev(q) = rev(a)·inv mod x^L (nq ≥ 2L - 1: no wrap into the low L words), reversed into q
+  int rc = RONK_OK;
+  RONK_TRY(reverse_rows(ctx, a, da, da - 1, L, X, nq, nq, batch));
+  RONK_TRY(rows_fold(ctx, f, G, L, L, d.lq, d.rows_b, B));
+  const u64* QR = rows_product(ctx, p, g, X, B, d.lq, batch, b_shared, &rc);
+  RONK_TRY(rc);
+  RONK_TRY(reverse_rows(ctx, QR, nq, L - 1, L, q, da, da, batch));
+  if (rw == 0) {
+    RONK_CUDA(ctx, cudaMemsetAsync(r, 0, (size_t)batch * da * sizeof(u64), ctx->stream));
+    return RONK_OK;
+  }
+  // (3) r = a - b·q on its low rw words: (b mod x^rw)·(q mod x^rw) when L ≥ rw (nr ≥ 2·rw - 1, no wrap), else b·q and a
+  // mod x^nr - 1 (nr ≥ rw > L), the cyclic difference being r itself
+  const u64 total = (u64)batch * nr;
+  RONK_TRY(launch(ctx, "poly_rows_pad", poly_rows_pad_kernel, grid_for(ctx, total, PAD_THREADS), PAD_THREADS, 0, false, (const u64*)q,
+                  (u32)std::min(L, rw), (u64)da, d.lr, total, X));
+  RONK_TRY(rows_fold(ctx, f, b, db, L >= rw ? rw : db, d.lr, d.rows_b, B));
+  const u64* P = rows_product(ctx, p, g, X, B, d.lr, batch, b_shared, &rc);
+  RONK_TRY(rc);
+  const u64 words = (u64)batch * da;
+  return launch(ctx, "divrem_rows_rem", divrem_rows_rem_kernel<F>, grid_for(ctx, words, 256), 256, 0, false, f, a, da,
+                L >= rw ? da : nr, P, nr, rw, words, r);
+}
+
+int divrem_newton_rows(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, bool b_shared, u32 batch,
+                       u64 top, u64* q, u64* r) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return divrem_newton_rows_with_field(ctx, f, p, g, a, da, b, db, b_shared, batch, top, q, r);
+  });
+}
+
+int divrem_top_inverses(ronk_ctx* ctx, u64 p, const u64* b, size_t db, u32 batch, u64* out) {
+  return with_field(ctx, p, 0, false, [&](const auto& f) {
+    return launch(ctx, "divrem_top_inv", divrem_top_inv_kernel<std::decay_t<decltype(f)>>, grid_for(ctx, batch, 256), 256, 0, false,
+                  f, b, db, batch, out, (size_t)2, true);
+  });
+}
+
 }  // namespace ronk

@@ -100,6 +100,9 @@ struct ronk_tune {
   int poly_batch_path = 0;  // RONK_POLY_BATCH_PATH: path of ronk_poly_mul_batch_u64 where it applies: 0 = the measured crossovers,
                             // 1 = schoolbook, 2 = transforms (fused up to its cap, multi-modular where no root fits), 3 = the
                             // batched transforms even where the fused kernel fits (poly_batch.cu)
+  int divrem_batch_path = 0;  // RONK_DIVREM_BATCH_PATH: path of ronk_poly_divrem_batch_u64 from batch 2, for rows with nonzero
+                              // top words and da ≥ db > 2: 0 = the measured rule, 1 = the literal kernel, 2 = Newton iteration
+                              // wherever its transforms fit (poly.cu)
 };
 
 struct ronk_ctx {
@@ -451,6 +454,16 @@ int poly_eval_device(ronk_ctx* ctx, u64 p, const u64* c, size_t d, const u64* xs
 bool divrem_newton_fits(u64 p, u64 g, size_t da, size_t db);  // poly_div.cu
 int divrem_newton_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, u64 top, u64* q,
                          u64* r);
+// poly_div.cu, batches of rows (a, q, r: batch × da; b: batch × db, or db words when b_shared), top words nonzero:
+// divrem_newton_rows runs Newton iteration on batched transforms (top = the shared divisor's top word; arguments checked
+// by the caller, batch ≥ 2, scratch reserved from divrem_newton_rows_scratch; stream-ordered).
+// divrem_newton_rows_transform_words: batch × the plan's larger transform.  divrem_top_inverses: out[2y] = b_y[db-1]^-1,
+// out[2y + 1] = -b_y[0]·out[2y], one launch profiled as divrem_top_inv.
+int divrem_newton_rows(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, const u64* b, size_t db, bool b_shared, u32 batch,
+                       u64 top, u64* q, u64* r);
+size_t divrem_newton_rows_scratch(size_t da, size_t db, bool b_shared, u32 batch);
+u64 divrem_newton_rows_transform_words(size_t da, size_t db, u32 batch);
+int divrem_top_inverses(ronk_ctx* ctx, u64 p, const u64* b, size_t db, u32 batch, u64* out);
 // G = hr^-1 mod x^L (hr: hl ≤ L words, g1 = hr[0]^-1); X, Y: 2^⌈log2(2L - 1)⌉ words each.  Stream-ordered.
 int newton_inverse_device(ronk_ctx* ctx, u64 p, u64 g, const u64* hr, size_t hl, size_t L, u64 g1, u64* G, u64* X, u64* Y);
 // Subproduct tree (poly_tree.cu) over k ≤ kTreeMaxLeaves points.  tree_fits: g != 0 and every transform of the plan

@@ -47,6 +47,27 @@ def open_(coeffs, eval_point, g1_srs) -> AffinePoint:
     return commit([int(v) for v in q.coefficients], g1_srs)
 
 
+def open_batch(polys, eval_point, g1_srs) -> list:
+    """open_ of every polynomial at one point: the quotients by the shared divisor [-z, 1] in one batched division
+    (ronk_poly_divrem_batch_u64_host), then one commit per quotient.  Returns the points
+    [open_(f, eval_point, g1_srs) for f in polys].  The rows of one batched call share their length, so polynomials of
+    different lengths take one call per length rather than being zero-padded to one: a quotient keeps its polynomial's
+    length, and that length sets how many SRS points commit uses (and checks against len(g1_srs))."""
+    rows = [Polynomial(f, PlutoScalarField) for f in polys]
+    z = PlutoScalarField(getattr(eval_point, "value", eval_point))
+    divisor = np.array([(-z).value, 1], dtype=np.uint64)
+    quotients = [None] * len(rows)
+    for d in sorted({len(f.coefficients) for f in rows}):
+        idx = [i for i, f in enumerate(rows) if len(f.coefficients) == d]
+        a = np.ascontiguousarray(np.stack([rows[i].coefficients for i in idx]), dtype=np.uint64)
+        q, r = np.empty_like(a), np.empty_like(a)
+        _lib.default_context().call("ronk_poly_divrem_batch_u64_host", rows[idx[0]].p, 0, _lib._ptr(a), d, _lib._ptr(divisor), 2, 1,
+                                    len(idx), _lib._ptr(q), _lib._ptr(r))
+        for i, row in zip(idx, q):
+            quotients[i] = row
+    return [commit([int(v) for v in q], g1_srs) for q in quotients]
+
+
 def commit_lagrange(evaluations, g1_srs) -> AffinePoint:
     """Commit to a polynomial given in the LAGRANGE basis over the 2^k-th roots of unity of F17 — the form in
     which the PLONK compiler emits its selector / permutation polynomials (compiler/program.rs:118-226,

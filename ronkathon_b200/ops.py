@@ -107,6 +107,23 @@ def poly_divrem(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
     return q, r
 
 
+def poly_divrem_batch(ctx: Context, a, b, p: int = GOLDILOCKS, g: int = 7):
+    """Polynomial::quotient_and_remainder of every row: a is (batch, da); b is (batch, db), or (db,) for one divisor
+    shared by every row.  Returns new (q, r) tensors of shape (batch, da), each row the words poly_divrem gives for it.
+    Synchronous; raises RonkPanic where the reference panics on any row."""
+    import torch
+    _check_u64(a); _check_u64(b)
+    assert a.dim() == 2 and b.dim() in (1, 2), "a is (batch, da); b is (batch, db) or (db,)"
+    batch, da = a.shape
+    shared = b.dim() == 1
+    assert shared or b.shape[0] == batch
+    q = torch.empty_like(a)
+    r = torch.empty_like(a)
+    ctx.call("ronk_poly_divrem_batch_u64", p, g, _lib._ptr(a), da, _lib._ptr(b), b.shape[-1], int(shared), batch, _lib._ptr(q),
+             _lib._ptr(r))
+    return q, r
+
+
 def poly_eval(ctx: Context, coeffs, xs, p: int = GOLDILOCKS):
     import torch
     _check_u64(coeffs); _check_u64(xs)
