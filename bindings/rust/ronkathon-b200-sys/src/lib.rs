@@ -123,6 +123,9 @@ extern "C" {
   pub fn ronk_point_smul_pluto_ext_host(ctx: *mut ronk_ctx, a: *const u8, scalars: *const u8, out: *mut u8, n: usize) -> c_int;
   pub fn ronk_msm_pluto_ext(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, out: *mut u8) -> c_int;
   pub fn ronk_msm_pluto_ext_host(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, out: *mut u8) -> c_int;
+  /// `kzg::commit` of `batch` contiguous scalar rows against one SRS; device pointers, out is batch × 4 bytes on the device.
+  pub fn ronk_msm_pluto_ext_batch(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, batch: u32, out: *mut u8) -> c_int;
+  pub fn ronk_msm_pluto_ext_batch_host(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, batch: u32, out: *mut u8) -> c_int;
   pub fn ronk_msm_pluto_ext_buckets(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, buckets: *mut u8) -> c_int;
   pub fn ronk_msm_combine_buckets_host(ctx: *mut ronk_ctx, buckets: *const u8, n_sets: usize, out: *mut u8) -> c_int;
 

@@ -495,6 +495,32 @@ int ronk_point_smul_pluto_ext_host(ronk_ctx *ctx, const uint8_t *a, const uint8_
  * buffer; synchronous. */
 int ronk_msm_pluto_ext(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t out[4]);
 int ronk_msm_pluto_ext_host(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t out[4]);
+/* `batch` commitments against one SRS (kzg::commit of many coefficient rows: a prover's columns, the quotients of
+ * kzg.open_batch).  scalars is batch × n_scalars bytes, row-major, rows contiguous with no padding and no stride; out is
+ * batch × 4 bytes in the packed point format above.  All pointers are DEVICE pointers.
+ * - Words: out[4r .. 4r+4) is exactly the point ronk_msm_pluto_ext(points, n_points, scalars + r·n_scalars, n_scalars)
+ *   returns, for every r < batch.
+ * - Errors, in this order: (1) without reading memory: RONK_EINVAL for a null ctx, a null points or scalars when
+ *   batch·n_scalars > 0, a null out when batch > 0, n_points < n_scalars (the reference's assert, kzg/setup.rs:53), or
+ *   points or out not 4-byte aligned (scalars may have any alignment); RONK_EUNSUPPORTED for batch·n_scalars above 2^40
+ *   bytes; (2) RONK_EINVAL when out overlaps points[0, 4·n_scalars) or the scalar block; (3) scratch (RONK_ENOMEM) is
+ *   taken before the first launch; (4) the call runs, then RONK_EINVAL if any of the first n_scalars points is off the
+ *   curve or non-canonical, or any scalar of any row is ≥ 17, with out not written (the last launch decides that on the
+ *   device).  After (1) and (2) nothing has been enqueued or written.  batch == 0 does nothing; n_scalars == 0 writes
+ *   Infinity to every row (the empty sum, curve/mod.rs:219-223), with one memset.
+ * - Launches, three whatever the batch: msm_coord_pack looks up each of the first n_scalars points' group coordinates
+ *   (a_i, b_i) once and writes them as two byte planes; msm_rows streams the scalar rows once and takes each row's
+ *   Σ s_i·a_i and Σ s_i·b_i mod 102 per column of 2048 scalars by __dp4a, four terms at a time; msm_rows_finish sums each
+ *   row's columns and looks the point up.  The group tables are built once per context on first use, by either commit
+ *   entry.  RONK_MSM_COORD, RONK_MSM_HIST and RONK_MSM_SPLIT select paths for ronk_msm_pluto_ext only.
+ * - Scratch: 2·⌈n_scalars/16⌉·16 bytes of planes and 4·batch·⌈n_scalars/2048⌉ bytes of column sums.
+ * - Synchronises once, to read the error flag, as ronk_msm_pluto_ext does.  The _host twin makes the checks of (1) but
+ *   the alignment check (its staging aligns the device buffers) before it stages anything, ships only the first
+ *   n_scalars points, stages in and out and synchronises. */
+int ronk_msm_pluto_ext_batch(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars,
+                             size_t n_scalars, uint32_t batch, uint8_t *out);
+int ronk_msm_pluto_ext_batch_host(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars,
+                                  size_t n_scalars, uint32_t batch, uint8_t *out);
 /* Per-device partial MSM for the multi-GPU path: writes the 17 bucket sums (17×4 bytes, host)
  * so ranks can combine them; ronk_msm_combine_buckets folds world×17 buckets into one point. */
 int ronk_msm_pluto_ext_buckets(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t buckets[68]);

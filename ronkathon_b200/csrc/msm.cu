@@ -310,11 +310,8 @@ constexpr int MSM_COORD_U = 2;  // 16-byte point loads per thread and batch; two
 
 // Branch-free: a rejected term only raises `bad` (the call then fails and the sums are discarded).
 __device__ __forceinline__ void msm_coord_term(u32 w, u32 s, const u32* __restrict__ tab, u32& acc_a, u32& acc_b, u32& bad) {
-  // every coordinate < 101  ⟺  no byte of w or of w + 27·0x01010101 has bit 7 set (bytes < 128 cannot carry into their
-  // neighbour); Infinity (0xFFFFFFFF) is not canonical and contributes nothing
-  const bool canon = ((w | (w + 0x1B1B1B1Bu)) & 0x80808080u) == 0u;
-  const u32 e = canon ? tab[pt_bin(w)] : 0xFFFFFFFFu;
-  const bool on = canon && (e & 0xFFFFu) == (w >> 16);   // on y² = x³ + 3 (empty bins hold 0xFFFF in the y field)
+  u32 e;
+  const bool on = coord_term(w, tab, e);                 // Infinity contributes nothing
   bad |= (u32)(s >= 17u) | (u32)(!on && w != PT_INF);    // not an F17 residue / off the curve / non-canonical
   const u32 sv = on ? s : 0u;                            // s = 0 adds nothing: g1 * 0 = Infinity (curve/mod.rs:163-165)
   acc_a += sv * ((e >> 16) & 0xFFu);
@@ -413,22 +410,28 @@ msm_coord_kernel(const u32* __restrict__ points, const uint8_t* __restrict__ sca
   }
 }
 
+// ctx->msm_coord: bintab[kTabWords] | pttab[102²] | counter, Σa, Σb — built once per context, on first use by either commit
+// entry (basis search + tables on the host, ≈ 3·10⁴ affine additions)
+constexpr size_t kTabWords = (MSM_BINS + 3) / 4 * 4;
+static int msm_coord_tables(ronk_ctx* ctx) {
+  if (ctx->msm_coord) return RONK_OK;
+  std::vector<u32> tabs(kTabWords + MSM_EXP * MSM_EXP + 4, 0xFFFFFFFFu);
+  if (!build_group_tables(tabs.data(), tabs.data() + kTabWords)) return set_err(ctx, RONK_ECUDA, "internal: no basis of E(F_101^2) found");
+  tabs[kTabWords + MSM_EXP * MSM_EXP + 0] = tabs[kTabWords + MSM_EXP * MSM_EXP + 1] = tabs[kTabWords + MSM_EXP * MSM_EXP + 2] = 0u;
+  RONK_CUDA(ctx, cudaMalloc(&ctx->msm_coord, tabs.size() * sizeof(u32)));
+  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->msm_coord, tabs.data(), tabs.size() * sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // tabs is pageable and goes out of scope
+  return RONK_OK;
+}
+
 static int msm_coord_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars, size_t n_scalars,
                             u32* h_result) {
   if (!ctx || (n_scalars && (!points || !scalars))) return set_err(ctx, RONK_EINVAL, "null argument");
   if (n_points < n_scalars) return set_err(ctx, RONK_EINVAL, "srs shorter than coefficients (kzg/setup.rs:53)");
   if (((uintptr_t)points & 3) != 0) return set_err(ctx, RONK_EINVAL, "points must be 4-byte aligned");
   if (n_scalars == 0) { *h_result = PT_INF; return RONK_OK; }   // empty sum = Infinity (curve/mod.rs:219-223)
-  constexpr size_t kTabWords = (MSM_BINS + 3) / 4 * 4;
   constexpr size_t kSmem = kTabWords * sizeof(u32);
-  if (!ctx->msm_coord) {  // one-time per context: basis search + tables on the host (≈ 3·10⁴ affine additions)
-    std::vector<u32> tabs(kTabWords + MSM_EXP * MSM_EXP + 4, 0xFFFFFFFFu);
-    if (!build_group_tables(tabs.data(), tabs.data() + kTabWords)) return set_err(ctx, RONK_ECUDA, "internal: no basis of E(F_101^2) found");
-    tabs[kTabWords + MSM_EXP * MSM_EXP + 0] = tabs[kTabWords + MSM_EXP * MSM_EXP + 1] = tabs[kTabWords + MSM_EXP * MSM_EXP + 2] = 0u;
-    RONK_CUDA(ctx, cudaMalloc(&ctx->msm_coord, tabs.size() * sizeof(u32)));
-    RONK_CUDA(ctx, cudaMemcpyAsync(ctx->msm_coord, tabs.data(), tabs.size() * sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
-    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // tabs is pageable and goes out of scope
-  }
+  RONK_TRY(msm_coord_tables(ctx));
   RONK_TRY(ensure_smem_attr(ctx, msm_coord_kernel, (int)kSmem));
   const u32* bintab = (const u32*)ctx->msm_coord;
   const u32* pttab = bintab + kTabWords;
@@ -447,6 +450,189 @@ static int msm_coord_device(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (host[0]) return set_err(ctx, RONK_EINVAL, "off-curve point, non-canonical coordinate or scalar >= 17");
   *h_result = host[1];
+  return RONK_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// kzg::commit of `batch` scalar rows against one SRS (ronk_msm_pluto_ext_batch).  The rows share the points, so each
+// point's group coordinates (a_i, b_i) are looked up and checked once per call, not once per row and point; a row is then
+// two byte dot products mod 102, four terms per __dp4a (scalars < 17, coordinates < 102).  Three launches whatever the
+// batch:
+//   msm_coord_pack_kernel   the first n points → byte planes A[i] = a_i, B[i] = b_i, zero-padded to a multiple of 16 bytes
+//                           (Infinity and rejected points: 0); raises the error flag for a bad point
+//   msm_rows_kernel         one warp per item of MSM_ROWS_R rows × one column of MSM_ROWS_CHUNK scalar words: each row's
+//                           (Σ s·a, Σ s·b) mod 102 over the column → partial[row][column]; raises the flag for a scalar
+//                           ≥ 17.  A plane word is loaded once per item and serves all its rows; the planes (2n bytes)
+//                           stay in L2 across rows, so the kernel streams the batch·n scalar bytes once
+//   msm_rows_finish_kernel  one warp per row: the row's partials mod 102 in a fixed order, then pttab[102·Σa + Σb] →
+//                           out[row], unless the flag is raised
+constexpr int MSM_PACK_THREADS = 256;
+constexpr int MSM_ROWS_THREADS = 256;
+constexpr int MSM_ROWS_R = 4;                      // rows per warp item
+constexpr int MSM_ROWS_U = 16;                     // scalar words per lane and row in one item
+constexpr u64 MSM_ROWS_CHUNK = 32 * MSM_ROWS_U;    // scalar words per column
+// Each __dp4a adds at most 4·16·101 = 6464 (four scalars < 17 times coordinates < 102); a lane's accumulators start at 0
+// in every item and are folded mod 102 at its end, after at most MSM_ROWS_U steps.
+static_assert((u64)MSM_ROWS_U * 6464u < (1ull << 32), "msm_rows_kernel's accumulators must not overflow between folds");
+
+__global__ void __launch_bounds__(MSM_PACK_THREADS)
+msm_coord_pack_kernel(const u32* __restrict__ points, size_t n, size_t plane_words, const u32* __restrict__ bintab,
+                      u32* __restrict__ A, u32* __restrict__ B, volatile u32* flag) {
+  const size_t stride = (size_t)gridDim.x * MSM_PACK_THREADS;
+  u32 bad = 0;
+  for (size_t k = (size_t)blockIdx.x * MSM_PACK_THREADS + threadIdx.x; k < plane_words; k += stride) {
+    u32 a4 = 0, b4 = 0;
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const size_t i = 4 * k + j;
+      if (i >= n) break;
+      const u32 w = points[i];
+      u32 e;
+      const bool on = coord_term(w, bintab, e);
+      bad |= (u32)(!on && w != PT_INF);   // off the curve / non-canonical
+      if (on) {
+        a4 |= ((e >> 16) & 0xFFu) << (8 * j);
+        b4 |= (e >> 24) << (8 * j);
+      }
+    }
+    A[k] = a4;
+    B[k] = b4;
+  }
+  if (bad) *flag = 1u;
+}
+
+__global__ void __launch_bounds__(MSM_ROWS_THREADS, 4)
+msm_rows_kernel(const uint8_t* __restrict__ scalars, size_t n, u32 batch, const u32* __restrict__ A, const u32* __restrict__ B,
+                u64 cols, u32* __restrict__ partial, volatile u32* flag) {
+  const u32 lane = threadIdx.x & 31u;
+  const u64 items = ((u64)batch + MSM_ROWS_R - 1) / MSM_ROWS_R * cols;
+  const u64 warps = (u64)gridDim.x * (MSM_ROWS_THREADS / 32);
+  const u64 full = n >> 2, words = (n + 3) >> 2;   // whole scalar words of a row; with its byte tail
+  u32 bad = 0;
+  for (u64 item = (u64)blockIdx.x * (MSM_ROWS_THREADS / 32) + (threadIdx.x >> 5); item < items; item += warps) {
+    const u64 grp = item / cols, col = item - grp * cols;
+    const u64 r0 = grp * MSM_ROWS_R;
+    u32 acc_a[MSM_ROWS_R], acc_b[MSM_ROWS_R];
+#pragma unroll
+    for (int j = 0; j < MSM_ROWS_R; j++) acc_a[j] = acc_b[j] = 0u;
+#pragma unroll 4
+    for (int u = 0; u < MSM_ROWS_U; u++) {
+      const u64 k = col * MSM_ROWS_CHUNK + (u64)u * 32u + lane;
+      if (k >= words) break;
+      const u32 a4 = A[k], b4 = B[k];
+#pragma unroll
+      for (int j = 0; j < MSM_ROWS_R; j++) {
+        if (r0 + j >= batch) break;
+        // row r starts at byte r·n, so most rows are not 4-byte aligned: word k of the row is the funnel shift of the two
+        // aligned words it straddles.  The upper one holds a byte of the row whenever the shift is nonzero, so no load
+        // leaves the scalar block.  The row's last n mod 4 scalars are read as bytes.
+        const uint8_t* row = scalars + (r0 + j) * n;
+        u32 s4 = 0;
+        if (k < full) {
+          const uintptr_t at = (uintptr_t)(row + 4 * k);
+          const u32 sh = (u32)(at & 3u);
+          const u32* wp = reinterpret_cast<const u32*>(at - sh);
+          s4 = __funnelshift_r(wp[0], sh ? wp[1] : 0u, 8u * sh);
+        } else {
+          for (u32 t = 0; t < (u32)(n & 3u); t++) s4 |= (u32)row[4 * k + t] << (8u * t);
+        }
+        bad |= scalar4_over(s4);
+        acc_a[j] = __dp4a(s4, a4, acc_a[j]);
+        acc_b[j] = __dp4a(s4, b4, acc_b[j]);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < MSM_ROWS_R; j++) {
+      u32 a = acc_a[j] % MSM_EXP, b = acc_b[j] % MSM_EXP;
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) {
+        a += __shfl_down_sync(0xFFFFFFFFu, a, off);
+        b += __shfl_down_sync(0xFFFFFFFFu, b, off);
+      }
+      if (lane == 0 && r0 + j < batch) partial[(r0 + j) * cols + col] = (a % MSM_EXP) | ((b % MSM_EXP) << 16);
+    }
+  }
+  if (bad) *flag = 1u;
+}
+
+__global__ void __launch_bounds__(MSM_ROWS_THREADS)
+msm_rows_finish_kernel(const u32* __restrict__ partial, u64 cols, u32 batch, const u32* __restrict__ pttab,
+                       const volatile u32* flag, u32* __restrict__ out) {
+  __shared__ u32 raised;
+  if (threadIdx.x == 0) raised = *flag;   // the earlier launches of the call have completed: one read per CTA
+  __syncthreads();
+  if (raised) return;                     // a rejected call leaves out as it was
+  const u32 lane = threadIdx.x & 31u;
+  const u64 warps = (u64)gridDim.x * (MSM_ROWS_THREADS / 32);
+  for (u64 r = (u64)blockIdx.x * (MSM_ROWS_THREADS / 32) + (threadIdx.x >> 5); r < batch; r += warps) {
+    u32 sa = 0, sb = 0;
+    for (u64 c = lane; c < cols; c += 32) {
+      const u32 v = partial[r * cols + c];
+      sa += v & 0xFFFFu;
+      sb += v >> 16;
+      sa = sa >= MSM_EXP ? sa - MSM_EXP : sa;
+      sb = sb >= MSM_EXP ? sb - MSM_EXP : sb;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      sa += __shfl_down_sync(0xFFFFFFFFu, sa, off);
+      sb += __shfl_down_sync(0xFFFFFFFFu, sb, off);
+    }
+    if (lane == 0) out[r] = pttab[MSM_EXP * (sa % MSM_EXP) + sb % MSM_EXP];
+  }
+}
+
+static bool bytes_overlap(const void* x, size_t nx, const void* y, size_t ny) {
+  const uintptr_t a = (uintptr_t)x, b = (uintptr_t)y;
+  return nx && ny && a < b + ny && b < a + nx;
+}
+
+// Step (1) of ronk_msm_pluto_ext_batch's errors: the checks that read no memory.  The _host twin skips the alignment
+// check, which concerns the device buffers its staging provides.
+static int msm_batch_args(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars, size_t n_scalars,
+                          u32 batch, const uint8_t* out, bool device) {
+  if (!ctx) return RONK_EINVAL;
+  if ((batch && n_scalars && (!points || !scalars)) || (batch && !out)) return set_err(ctx, RONK_EINVAL, "null argument");
+  if (n_points < n_scalars) return set_err(ctx, RONK_EINVAL, "srs shorter than coefficients (kzg/setup.rs:53)");
+  if (device && ((((uintptr_t)points | (uintptr_t)out) & 3) != 0))
+    return set_err(ctx, RONK_EINVAL, "points and out must be 4-byte aligned");
+  if (batch && n_scalars > ((size_t)1 << 40) / batch) return set_err(ctx, RONK_EUNSUPPORTED, "batch * n_scalars above 2^40 bytes");
+  return RONK_OK;
+}
+
+static int msm_batch_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars, size_t n_scalars,
+                            u32 batch, uint8_t* out) {
+  RONK_TRY(msm_batch_args(ctx, points, n_points, scalars, n_scalars, batch, out, true));
+  if (bytes_overlap(out, (size_t)batch * 4, points, n_scalars * 4) || bytes_overlap(out, (size_t)batch * 4, scalars, (size_t)batch * n_scalars))
+    return set_err(ctx, RONK_EINVAL, "out overlaps the points or the scalars");
+  if (batch == 0) return RONK_OK;
+  if (n_scalars == 0) {  // every row is the empty sum, Infinity (curve/mod.rs:219-223)
+    RONK_CUDA(ctx, cudaMemsetAsync(out, 0xFF, (size_t)batch * 4, ctx->stream));
+    return RONK_OK;
+  }
+  RONK_TRY(msm_coord_tables(ctx));
+  const u32* bintab = (const u32*)ctx->msm_coord;
+  const u32* pttab = bintab + kTabWords;
+  const size_t plane_words = (n_scalars + 15) / 16 * 4;   // each plane: ⌈n/16⌉·16 bytes
+  const u64 cols = ((n_scalars + 3) / 4 + MSM_ROWS_CHUNK - 1) / MSM_ROWS_CHUNK;
+  const u64 items = ((u64)batch + MSM_ROWS_R - 1) / MSM_ROWS_R * cols;
+  Frame fr(ctx);
+  u32 *A = nullptr, *partial = nullptr;
+  RONK_TRY(fr.take(&A, 2 * plane_words));
+  RONK_TRY(fr.take(&partial, (size_t)batch * cols));
+  u32* B = A + plane_words;
+  volatile u32* host = (volatile u32*)ctx->h_flag;  // mapped pinned: [0] = flag
+  host[0] = 0u;
+  u32* flag = nullptr;
+  RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&flag, (void*)ctx->h_flag, 0));
+  RONK_TRY(launch(ctx, "msm_coord_pack", msm_coord_pack_kernel, grid_for(ctx, plane_words, MSM_PACK_THREADS), MSM_PACK_THREADS, 0,
+                  false, (const u32*)points, n_scalars, plane_words, bintab, A, B, (volatile u32*)flag));
+  RONK_TRY(launch(ctx, "msm_rows", msm_rows_kernel, grid_for(ctx, items, MSM_ROWS_THREADS / 32, 4), MSM_ROWS_THREADS, 0, false,
+                  scalars, n_scalars, batch, (const u32*)A, (const u32*)B, cols, partial, (volatile u32*)flag));
+  RONK_TRY(launch(ctx, "msm_rows_finish", msm_rows_finish_kernel, grid_for(ctx, batch, MSM_ROWS_THREADS / 32), MSM_ROWS_THREADS, 0,
+                  false, (const u32*)partial, cols, batch, pttab, (const volatile u32*)flag, (u32*)out));
+  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (host[0]) return set_err(ctx, RONK_EINVAL, "off-curve point, non-canonical coordinate or scalar >= 17");
   return RONK_OK;
 }
 
@@ -606,6 +792,27 @@ int ronk_msm_pluto_ext_host(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   RONK_TRY(stage_in(fr, s));
   return stage_out(
       ctx, ronk_msm_pluto_ext(ctx, (const uint8_t*)s[0].dev, n_scalars, (const uint8_t*)s[1].dev, n_scalars, out), s);
+}
+
+int ronk_msm_pluto_ext_batch(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars, size_t n_scalars,
+                             uint32_t batch, uint8_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  return msm_batch_device(ctx, points, n_points, scalars, n_scalars, batch, out);
+}
+
+// Ships only the first n_scalars points, as ronk_msm_pluto_ext_host does.
+int ronk_msm_pluto_ext_batch_host(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars,
+                                  size_t n_scalars, uint32_t batch, uint8_t* out) {
+  ronk::DeviceGuard _dg(ctx);
+  RONK_TRY(msm_batch_args(ctx, points, n_points, scalars, n_scalars, batch, out, false));
+  if (batch == 0) return RONK_OK;
+  Staged s[] = {{n_scalars * 4, points}, {(size_t)batch * n_scalars, scalars}, {(size_t)batch * 4, nullptr, out}};
+  Frame fr(ctx);
+  RONK_TRY(stage_in(fr, s));
+  return stage_out(ctx,
+                   ronk_msm_pluto_ext_batch(ctx, (const uint8_t*)s[0].dev, n_scalars, (const uint8_t*)s[1].dev, n_scalars, batch,
+                                            (uint8_t*)s[2].dev),
+                   s);
 }
 
 int ronk_msm_combine_buckets_host(ronk_ctx* ctx, const uint8_t* buckets, size_t n_sets, uint8_t out[4]) {

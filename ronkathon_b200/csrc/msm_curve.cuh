@@ -121,6 +121,19 @@ constexpr u32 MSM_EXP = 102;          // group exponent of E(F_101²) ≅ (Z/102
 RONK_DEV u32 y_bit(u32 y0, u32 y1) { return y0 ? (y0 > 50u) : (y1 > 50u); }
 RONK_DEV u32 pt_bin(u32 w) { return 2u * ((w & 0xFF) + Q101 * ((w >> 8) & 0xFF)) + y_bit((w >> 16) & 0xFF, w >> 24); }
 
+// The term test of the group-coordinate commit: whether the packed point w is canonical and on y² = x³ + 3
+// (curve/mod.rs:130-139), with e = its bintab entry (y0 | y1 << 8 | a << 16 | b << 24; 0xFFFFFFFF when w is not
+// canonical).  Every coordinate < 101  ⟺  no byte of w or of w + 27·0x01010101 has bit 7 set (bytes < 128 cannot carry
+// into their neighbour); Infinity (0xFFFFFFFF) is not canonical and is reported as not on the curve.
+RONK_DEV bool coord_term(u32 w, const u32* tab, u32& e) {
+  const bool canon = ((w | (w + 0x1B1B1B1Bu)) & 0x80808080u) == 0u;
+  e = canon ? tab[pt_bin(w)] : 0xFFFFFFFFu;
+  return canon && (e & 0xFFFFu) == (w >> 16);   // empty bins hold 0xFFFF in the y field
+}
+// Nonzero iff some byte of the four packed scalars s4 is ≥ 17, i.e. not an F17 residue: a byte < 17 stays below 128 after
+// adding 111, and a byte ≥ 128 flags itself (its carry can only reach bytes above it, which the word is already flagged by).
+RONK_DEV u32 scalar4_over(u32 s4) { return (s4 | (s4 + 0x6F6F6F6Fu)) & 0x80808080u; }
+
 // ---- group coordinates (host only; plan building for msm_coord_kernel, also compiled by tests/emu) ----
 // E(F_101²): y² = x³ + 3 has 102² points and exponent 102, i.e. E ≅ (Z/102)².  With a basis (G1, G2) every point is
 // a·G1 + b·G2 for exactly one (a, b) ∈ (Z/102)², and Σ s_i·P_i = (Σ s_i a_i)·G1 + (Σ s_i b_i)·G2: the whole commit is two

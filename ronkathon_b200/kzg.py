@@ -1,5 +1,6 @@
 """Host-side mirror of ronkathon's kzg module (src/kzg/setup.rs): setup / commit / open.
-`commit` is the Pippenger bucket-MSM kernel in libronk_b200.so; `check` (pairing) is out of scope."""
+`commit` is the group-coordinate MSM kernel in libronk_b200.so, `commit_batch` its batched form; `check` (pairing) is
+out of scope."""
 from __future__ import annotations
 
 import numpy as np
@@ -38,6 +39,24 @@ def commit(coeffs, g1_srs) -> AffinePoint:
     return AffinePoint(out.tobytes())
 
 
+def commit_batch(rows, g1_srs) -> list:
+    """[commit(r, g1_srs) for r in rows] in one batched call (ronk_msm_pluto_ext_batch_host), the panics included.  The
+    rows are zero-padded to the longest: a zero scalar adds nothing, and the longest row is the one that sets the SRS
+    length check."""
+    sc = [[int(getattr(c, "value", c)) % 17 for c in r] for r in rows]
+    if not sc:
+        return []
+    n = max(len(r) for r in sc)
+    block = np.zeros((len(sc), n), dtype=np.uint8)
+    for i, r in enumerate(sc):
+        block[i, :len(r)] = r
+    pts = _pack(g1_srs)
+    out = np.empty((len(sc), 4), dtype=np.uint8)
+    _lib.default_context().call("ronk_msm_pluto_ext_batch_host", _lib._ptr(pts), len(pts) // 4, _lib._ptr(block), n, len(sc),
+                                _lib._ptr(out))
+    return [AffinePoint(w.tobytes()) for w in out]
+
+
 def open_(coeffs, eval_point, g1_srs) -> AffinePoint:
     """kzg/setup.rs:63-78: poly / (x - z) by Polynomial::div, then commit the quotient."""
     poly = Polynomial(coeffs, PlutoScalarField)
@@ -49,10 +68,10 @@ def open_(coeffs, eval_point, g1_srs) -> AffinePoint:
 
 def open_batch(polys, eval_point, g1_srs) -> list:
     """open_ of every polynomial at one point: the quotients by the shared divisor [-z, 1] in one batched division
-    (ronk_poly_divrem_batch_u64_host), then one commit per quotient.  Returns the points
+    (ronk_poly_divrem_batch_u64_host), then every quotient in one commit_batch.  Returns the points
     [open_(f, eval_point, g1_srs) for f in polys].  The rows of one batched call share their length, so polynomials of
-    different lengths take one call per length rather than being zero-padded to one: a quotient keeps its polynomial's
-    length, and that length sets how many SRS points commit uses (and checks against len(g1_srs))."""
+    different lengths take one division per length rather than being zero-padded to one: a quotient keeps its
+    polynomial's length."""
     rows = [Polynomial(f, PlutoScalarField) for f in polys]
     z = PlutoScalarField(getattr(eval_point, "value", eval_point))
     divisor = np.array([(-z).value, 1], dtype=np.uint64)
@@ -65,7 +84,7 @@ def open_batch(polys, eval_point, g1_srs) -> list:
                                     len(idx), _lib._ptr(q), _lib._ptr(r))
         for i, row in zip(idx, q):
             quotients[i] = row
-    return [commit([int(v) for v in q], g1_srs) for q in quotients]
+    return commit_batch(quotients, g1_srs)
 
 
 def commit_lagrange(evaluations, g1_srs) -> AffinePoint:
@@ -101,6 +120,25 @@ def open_lagrange(evaluations, eval_point, g1_srs) -> AffinePoint:
 
 def commit_preprocessed(polys: dict, g1_srs) -> dict:
     """Commitments to a `CommonPreprocessedInput` (compiler/program.rs:59-63: ql, qr, qm, qo, qc, s1, s2, s3),
-    each given as GROUP_ORDER evaluations."""
-    return {name: commit_lagrange(ev, g1_srs) for name, ev in polys.items()}
+    each given as GROUP_ORDER evaluations: commit_lagrange of every column, with the columns' inverse transforms as one
+    batched transform per length (one in all, as the columns share GROUP_ORDER) and their commitments in one
+    commit_batch."""
+    from .polynomial import Lagrange
+    cols = {}
+    for name, ev in polys.items():
+        poly = ev if isinstance(ev, Polynomial) else Polynomial(ev, PlutoScalarField, Lagrange)
+        if poly.basis is not Lagrange:
+            raise _lib.RonkPanic(1, "commit_preprocessed expects Lagrange-basis polynomials")
+        n = len(poly.coefficients)
+        if n & (n - 1):   # where [(); D.is_power_of_two() as usize - 1]: (polynomial/mod.rs:274)
+            raise _lib.RonkPanic(1, "D must be a power of two")
+        cols[name] = poly
+    mono = {}
+    for n in sorted({len(p.coefficients) for p in cols.values()}):
+        names = [k for k, p in cols.items() if len(p.coefficients) == n]
+        data = np.ascontiguousarray(np.stack([cols[k].coefficients for k in names]), dtype=np.uint64)
+        p0 = cols[names[0]]
+        _lib.default_context().call("ronk_ntt_u64_host", p0.p, p0.g, _lib._ptr(data), n.bit_length() - 1, len(names), 1)
+        mono.update(zip(names, data))
+    return dict(zip(polys, commit_batch([mono[k] for k in polys], g1_srs)))
 

@@ -291,6 +291,20 @@ def msm(ctx: Context, points, scalars) -> bytes:
     return out.tobytes()
 
 
+def msm_batch(ctx: Context, points, scalars):
+    """kzg::commit of every row of scalars (uint8 [batch, n]) against the device-resident packed points (uint8 [n', 4],
+    n' ≥ n): a new uint8 [batch, 4] device tensor, row r the point msm gives for scalars[r].  Synchronous; raises
+    RonkPanic where msm does on any row."""
+    import torch
+    assert points.is_cuda and points.dtype == torch.uint8 and points.is_contiguous()
+    assert scalars.is_cuda and scalars.dtype == torch.uint8 and scalars.dim() == 2 and scalars.is_contiguous(), \
+        "scalars is a contiguous uint8 (batch, n) tensor"
+    batch, n = scalars.shape
+    out = torch.empty((batch, 4), dtype=torch.uint8, device=scalars.device)
+    ctx.call("ronk_msm_pluto_ext_batch", _lib._ptr(points), points.numel() // 4, _lib._ptr(scalars), n, batch, _lib._ptr(out))
+    return out
+
+
 def msm_buckets(ctx: Context, points, scalars) -> bytes:
     out = np.empty(68, dtype=np.uint8)
     ctx.call("ronk_msm_pluto_ext_buckets", _lib._ptr(points), points.numel() // 4, _lib._ptr(scalars),
