@@ -126,6 +126,12 @@ extern "C" {
   /// `kzg::commit` of `batch` contiguous scalar rows against one SRS; device pointers, out is batch × 4 bytes on the device.
   pub fn ronk_msm_pluto_ext_batch(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, batch: u32, out: *mut u8) -> c_int;
   pub fn ronk_msm_pluto_ext_batch_host(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, batch: u32, out: *mut u8) -> c_int;
+  /// The reference's Tate pairing on n pairs of E[17]; out[2i], out[2i+1] = c0, c1.  Device pointers.
+  pub fn ronk_pairing_pluto_ext(ctx: *mut ronk_ctx, p: *const u8, q: *const u8, n: usize, out: *mut u8) -> c_int;
+  pub fn ronk_pairing_pluto_ext_host(ctx: *mut ronk_ctx, p: *const u8, q: *const u8, n: usize, out: *mut u8) -> c_int;
+  /// `kzg::check` of n openings against one SRS: ok[r] = 1 when the row verifies, else 0.  Device pointers.
+  pub fn ronk_kzg_check_pluto_ext_batch(ctx: *mut ronk_ctx, commitments: *const u8, proofs: *const u8, points: *const u8, values: *const u8, n: usize, g1_srs: *const u8, n_g1: usize, g2_srs: *const u8, n_g2: usize, ok: *mut u8) -> c_int;
+  pub fn ronk_kzg_check_pluto_ext_batch_host(ctx: *mut ronk_ctx, commitments: *const u8, proofs: *const u8, points: *const u8, values: *const u8, n: usize, g1_srs: *const u8, n_g1: usize, g2_srs: *const u8, n_g2: usize, ok: *mut u8) -> c_int;
   pub fn ronk_msm_pluto_ext_buckets(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, buckets: *mut u8) -> c_int;
   pub fn ronk_msm_combine_buckets_host(ctx: *mut ronk_ctx, buckets: *const u8, n_sets: usize, out: *mut u8) -> c_int;
 

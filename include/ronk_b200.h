@@ -521,6 +521,41 @@ int ronk_msm_pluto_ext_batch(ronk_ctx *ctx, const uint8_t *points, size_t n_poin
                              size_t n_scalars, uint32_t batch, uint8_t *out);
 int ronk_msm_pluto_ext_batch_host(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars,
                                   size_t n_scalars, uint32_t batch, uint8_t *out);
+/* The reference's Tate pairing (curve/pairing.rs:33-54) of PlutoExtendedCurve with R = 17 on n pairs:
+ * out[2i], out[2i+1] = c0, c1 of pairing(p[i], q[i]) ∈ GF(101²).  And kzg::check (kzg/setup.rs:81-103) of n openings
+ * against one SRS: ok[r] = 1 when pairing(proofs[r], g2_srs[1] − GEN·points[r]) == pairing(commitments[r] −
+ * g1_srs[0]·values[r], GEN), else 0, with GEN = PlutoExtendedCurve::GENERATOR (36, 31t).
+ * - Layout: points in the packed 4-byte format above, 0xFFFFFFFF is Infinity.  p, q, commitments and proofs are n × 4
+ *   bytes; points and values are n bytes each, F17 residues; out is 2n bytes, ok is n bytes; g1_srs holds n_g1 points
+ *   and g2_srs n_g2, of which the check reads only g1_srs[0] and g2_srs[1].  All pointers of the device entries are
+ *   DEVICE pointers.
+ * - Words: each output byte is exactly what the reference computes for its row.  Only points of E[17] pair: the 289
+ *   points a·G1 + b·G2 with 6 | a and 6 | b in a basis of E ≅ (Z/102)².  The literal Miller loop (zero-skipping, the
+ *   `zeros` counter, the final x^600) is run once per context on every pair of E[17] into an 83 521-byte table, built on
+ *   first use by either entry after the commit's group tables; its values are not bilinear, so nothing is derived from
+ *   a basis.  A row is then four coordinate lookups, a little arithmetic mod 102 and table lookups.
+ * - Errors, in this order: (1) without reading memory: RONK_EINVAL for a null ctx, a null pointer when n > 0, n_g1 == 0
+ *   or n_g2 < 2 (the reference's two panics, whatever n), or a point array (p, q, commitments, proofs, g1_srs, g2_srs)
+ *   not 4-byte aligned; RONK_EUNSUPPORTED for n ≥ 2^32; (2) RONK_EINVAL when an output overlaps an input (for the
+ *   check: commitments, proofs, points, values, g1_srs[0] or g2_srs[0..2)); (3) scratch and the one-time tables are
+ *   taken (RONK_ENOMEM / RONK_ECUDA); (4) the call runs, then RONK_EINVAL if any row panics in the reference or holds
+ *   input the ABI rejects: an off-curve or non-canonical point (for the check: a commitment, a proof, g1_srs[0] or
+ *   g2_srs[1]), a scalar ≥ 17; for the pairing an argument outside E[17], Infinity, or P == Q; for the check either
+ *   pairing panicking (the proof, g2_srs[1] − GEN·point or commitment − g1_srs[0]·value is Infinity or outside E[17],
+ *   or the pair is one of the table's panics).  After (1) and (2) nothing has been enqueued or written; after (4) the
+ *   output bytes are unspecified.  n == 0 does nothing.
+ * - Launches: one whatever n (kzg_check keeps both tables in shared memory; pairing reads them through L1), plus the
+ *   table build on a context's first call.  Synchronises once, to read the error flag, as ronk_msm_pluto_ext_batch does.
+ * - The _host twins make the checks of (1) but the alignment check (their staging aligns the device buffers) before they
+ *   stage anything; the check twin ships only g1_srs[0] and g2_srs[0..2). */
+int ronk_pairing_pluto_ext(ronk_ctx *ctx, const uint8_t *p, const uint8_t *q, size_t n, uint8_t *out);
+int ronk_pairing_pluto_ext_host(ronk_ctx *ctx, const uint8_t *p, const uint8_t *q, size_t n, uint8_t *out);
+int ronk_kzg_check_pluto_ext_batch(ronk_ctx *ctx, const uint8_t *commitments, const uint8_t *proofs,
+                                   const uint8_t *points, const uint8_t *values, size_t n,
+                                   const uint8_t *g1_srs, size_t n_g1, const uint8_t *g2_srs, size_t n_g2, uint8_t *ok);
+int ronk_kzg_check_pluto_ext_batch_host(ronk_ctx *ctx, const uint8_t *commitments, const uint8_t *proofs,
+                                        const uint8_t *points, const uint8_t *values, size_t n,
+                                        const uint8_t *g1_srs, size_t n_g1, const uint8_t *g2_srs, size_t n_g2, uint8_t *ok);
 /* Per-device partial MSM for the multi-GPU path: writes the 17 bucket sums (17×4 bytes, host)
  * so ranks can combine them; ronk_msm_combine_buckets folds world×17 buckets into one point. */
 int ronk_msm_pluto_ext_buckets(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t buckets[68]);

@@ -121,6 +121,7 @@ int ronk_ctx_destroy(ronk_ctx* ctx) {
   if (ctx->msm_ytab) cudaFree(ctx->msm_ytab);
   if (ctx->msm_done) cudaFree(ctx->msm_done);
   if (ctx->msm_coord) cudaFree(ctx->msm_coord);
+  if (ctx->pairing_tab) cudaFree(ctx->pairing_tab);
   if (ctx->d_flag) cudaFree(ctx->d_flag);
   if (ctx->h_flag) cudaFreeHost(ctx->h_flag);
   delete ctx;

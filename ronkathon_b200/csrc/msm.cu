@@ -411,9 +411,8 @@ msm_coord_kernel(const u32* __restrict__ points, const uint8_t* __restrict__ sca
 }
 
 // ctx->msm_coord: bintab[kTabWords] | pttab[102²] | counter, Σa, Σb — built once per context, on first use by either commit
-// entry (basis search + tables on the host, ≈ 3·10⁴ affine additions)
-constexpr size_t kTabWords = (MSM_BINS + 3) / 4 * 4;
-static int msm_coord_tables(ronk_ctx* ctx) {
+// entry or by the pairing table (basis search + tables on the host, ≈ 3·10⁴ affine additions)
+int msm_coord_tables(ronk_ctx* ctx) {
   if (ctx->msm_coord) return RONK_OK;
   std::vector<u32> tabs(kTabWords + MSM_EXP * MSM_EXP + 4, 0xFFFFFFFFu);
   if (!build_group_tables(tabs.data(), tabs.data() + kTabWords)) return set_err(ctx, RONK_ECUDA, "internal: no basis of E(F_101^2) found");
@@ -580,11 +579,6 @@ msm_rows_finish_kernel(const u32* __restrict__ partial, u64 cols, u32 batch, con
     }
     if (lane == 0) out[r] = pttab[MSM_EXP * (sa % MSM_EXP) + sb % MSM_EXP];
   }
-}
-
-static bool bytes_overlap(const void* x, size_t nx, const void* y, size_t ny) {
-  const uintptr_t a = (uintptr_t)x, b = (uintptr_t)y;
-  return nx && ny && a < b + ny && b < a + nx;
 }
 
 // Step (1) of ronk_msm_pluto_ext_batch's errors: the checks that read no memory.  The _host twin skips the alignment

@@ -141,9 +141,11 @@ RONK_DEV u32 scalar4_over(u32 s4) { return (s4 | (s4 + 0x6F6F6F6Fu)) & 0x8080808
 // additions (curve/mod.rs:178-213) arrives at, because the addition law is associative and commutative.
 //   bintab[bin(P)] = y0 | y1 << 8 | a << 16 | b << 24   (0xFFFFFFFF: no curve point in the bin — doubles as is_on_curve)
 //   pttab[102 a + b] = packed a·G1 + b·G2                (PT_INF at 0)
+// On the device the bintab is padded to kTabWords (a multiple of four words), with pttab after it (ctx->msm_coord).
 // The basis is found by search, deterministically (first points in x order that work), with the reference's own
 // addition law; injectivity of (a, b) → point is CHECKED while the table is filled, so a wrong basis cannot survive.
 // Returns false if no basis was found (cannot happen for this curve; the caller reports an internal error).
+constexpr u32 kTabWords = (MSM_BINS + 3) / 4 * 4;
 inline bool build_group_tables(u32* bintab /*MSM_BINS*/, u32* pttab /*MSM_EXP²*/) {
   // curve points in x order: sq[idx(y²)] = y
   static const u32 kNone = 0xFFFFFFFFu;

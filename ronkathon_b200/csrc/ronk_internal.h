@@ -130,6 +130,7 @@ struct ronk_ctx {
   void* msm_ytab = nullptr;  // uint16_t[20402]: y of the curve point in each histogram bin (msm.cu), built on first use
   void* msm_done = nullptr;  // u32 completion counter of msm_hist_finish_kernel
   void* msm_coord = nullptr; // msm_coord_kernel: bintab[20404] | pttab[10404] | counter, Σa, Σb (msm.cu), built on first use
+  void* pairing_tab = nullptr;  // uint8_t T[289²] of the Tate pairing on E[17], padded | μ17 list (pairing.cu), built on first use
   int* d_flag = nullptr;  // device error flag
   int* h_flag = nullptr;  // pinned host mirror: h_flag[0] = error flag, h_flag[1..31] = small results (msm.cu)
 };
@@ -382,6 +383,16 @@ inline int stage_out(ronk_ctx* ctx, int rc, const Staged (&r)[N]) {
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return RONK_OK;
 }
+
+// Whether the nx bytes at x and the ny bytes at y share a byte (never for a null or empty region).
+inline bool bytes_overlap(const void* x, size_t nx, const void* y, size_t ny) {
+  if (!x || !y || !nx || !ny) return false;
+  const uintptr_t a = (uintptr_t)x, b = (uintptr_t)y;
+  return a < b + ny && b < a + nx;
+}
+
+// ctx->msm_coord's group tables (msm.cu), built on the first call that needs them.
+int msm_coord_tables(ronk_ctx* ctx);
 
 // Whether the nx words at x and the ny words at y share a word.
 inline bool overlaps(const u64* x, size_t nx, const u64* y, size_t ny) { return nx && ny && x < y + ny && y < x + nx; }

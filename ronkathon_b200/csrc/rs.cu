@@ -327,12 +327,6 @@ rs_finish_kernel(const u64* __restrict__ C, u64 n, u64 k, const RsRow* __restric
   if (blockIdx.y == 0 && threadIdx.x == 0) status[b] = ok ? (int32_t)(rw.deg - rw.eps) : -1;
 }
 
-static bool bytes_overlap(const void* a, size_t na, const void* b, size_t nb) {
-  if (!a || !b || !na || !nb) return false;
-  const char *x = (const char*)a, *y = (const char*)b;
-  return x < y + nb && y < x + na;
-}
-
 // Checks shared by encode and decode, after the null checks: *path set on RONK_OK.  `rows` transforms of n points
 // run in one call; 3·batch·n < 2^31 is within what every transform path takes.
 static int rs_args(ronk_ctx* ctx, u64 p, u64 g, const void* in, u64 n, u64 k, u64 rows, AnyNttPath* path) {

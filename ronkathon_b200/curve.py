@@ -89,3 +89,13 @@ def sum_points(points):
     for p in points:
         acc = p if acc is None else acc + p
     return AffinePoint.infinity() if acc is None else acc
+
+
+def pairing(p: AffinePoint, q: AffinePoint):
+    """pairing::<PlutoExtendedCurve, 17> (curve/pairing.rs:33-54): (c0, c1) of the value in GF(101²), a 17th root of
+    unity.  Raises RonkPanic where the reference panics: p or q is not 17-torsion or is Infinity, or p == q."""
+    out = np.empty(2, dtype=np.uint8)
+    a = np.frombuffer(p.raw, dtype=np.uint8).copy()
+    b = np.frombuffer(q.raw, dtype=np.uint8).copy()
+    _lib.default_context().call("ronk_pairing_pluto_ext_host", _lib._ptr(a), _lib._ptr(b), 1, _lib._ptr(out))
+    return int(out[0]), int(out[1])

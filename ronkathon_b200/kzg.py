@@ -1,6 +1,6 @@
-"""Host-side mirror of ronkathon's kzg module (src/kzg/setup.rs): setup / commit / open.
-`commit` is the group-coordinate MSM kernel in libronk_b200.so, `commit_batch` its batched form; `check` (pairing) is
-out of scope."""
+"""Host-side mirror of ronkathon's kzg module (src/kzg/setup.rs): setup / commit / open / check.
+`commit` is the group-coordinate MSM kernel in libronk_b200.so, `commit_batch` its batched form; `check` and
+`check_batch` look both pairings up in a table of the reference's Tate pairing on E[17] (ronk_kzg_check_pluto_ext_batch)."""
 from __future__ import annotations
 
 import numpy as np
@@ -85,6 +85,31 @@ def open_batch(polys, eval_point, g1_srs) -> list:
         for i, row in zip(idx, q):
             quotients[i] = row
     return commit_batch(quotients, g1_srs)
+
+
+def _scalars(xs) -> np.ndarray:
+    return np.array([int(getattr(x, "value", x)) % 17 for x in xs], dtype=np.uint8)
+
+
+def check(p, q, point, value, g1_srs, g2_srs) -> bool:
+    """kzg/setup.rs:81-103: pairing(q, g2_srs[1] - GEN·point) == pairing(p - g1_srs[0]·value, GEN).  Raises RonkPanic
+    where the reference panics: an empty g1_srs, fewer than two g2_srs points, or either pairing panicking."""
+    return check_batch([p], [q], [point], [value], g1_srs, g2_srs)[0]
+
+
+def check_batch(commitments, proofs, points, values, g1_srs, g2_srs) -> list:
+    """[check(c, q, z, v, g1_srs, g2_srs) for each row] in one call (ronk_kzg_check_pluto_ext_batch_host); raises
+    RonkPanic if any row panics.  Scalars are reduced mod 17, as PlutoScalarField::new does."""
+    c, q = _pack(commitments), _pack(proofs)
+    z, v = _scalars(points), _scalars(values)
+    n = len(z)
+    if not (len(c) == len(q) == 4 * n and len(v) == n):
+        raise ValueError("commitments, proofs, points and values must have one entry per row")
+    g1, g2 = _pack(g1_srs), _pack(g2_srs)
+    ok = np.empty(n, dtype=np.uint8)
+    _lib.default_context().call("ronk_kzg_check_pluto_ext_batch_host", _lib._ptr(c), _lib._ptr(q), _lib._ptr(z), _lib._ptr(v), n,
+                                _lib._ptr(g1), len(g1) // 4, _lib._ptr(g2), len(g2) // 4, _lib._ptr(ok))
+    return [bool(b) for b in ok]
 
 
 def commit_lagrange(evaluations, g1_srs) -> AffinePoint:

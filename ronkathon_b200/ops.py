@@ -305,6 +305,34 @@ def msm_batch(ctx: Context, points, scalars):
     return out
 
 
+def pairing(ctx: Context, P, Q):
+    """The reference's Tate pairing (curve/pairing.rs:33-54) of the device-resident packed points P[i], Q[i] (uint8 [n, 4]):
+    a new uint8 [n, 2] device tensor of (c0, c1).  Synchronous; raises RonkPanic where the reference panics on any pair."""
+    import torch
+    for t in (P, Q):
+        assert t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()
+    n = P.numel() // 4
+    assert Q.numel() == 4 * n
+    out = torch.empty((n, 2), dtype=torch.uint8, device=P.device)
+    ctx.call("ronk_pairing_pluto_ext", _lib._ptr(P), _lib._ptr(Q), n, _lib._ptr(out))
+    return out
+
+
+def kzg_check(ctx: Context, C, Pi, z, v, g1_srs, g2_srs):
+    """kzg::check (kzg/setup.rs:81-103) of every row on device tensors: commitments C and proofs Pi (uint8 [n, 4]),
+    points z and values v (uint8 [n], F17 residues), the SRS points g1_srs and g2_srs (uint8 [k, 4]).  A new uint8 [n]
+    device tensor, 1 where the row verifies.  Synchronous; raises RonkPanic where the reference panics on any row."""
+    import torch
+    for t in (C, Pi, z, v, g1_srs, g2_srs):
+        assert t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()
+    n = z.numel()
+    assert C.numel() == Pi.numel() == 4 * n and v.numel() == n
+    ok = torch.empty(n, dtype=torch.uint8, device=z.device)
+    ctx.call("ronk_kzg_check_pluto_ext_batch", _lib._ptr(C), _lib._ptr(Pi), _lib._ptr(z), _lib._ptr(v), n, _lib._ptr(g1_srs),
+             g1_srs.numel() // 4, _lib._ptr(g2_srs), g2_srs.numel() // 4, _lib._ptr(ok))
+    return ok
+
+
 def msm_buckets(ctx: Context, points, scalars) -> bytes:
     out = np.empty(68, dtype=np.uint8)
     ctx.call("ronk_msm_pluto_ext_buckets", _lib._ptr(points), points.numel() // 4, _lib._ptr(scalars),

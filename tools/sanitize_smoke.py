@@ -7,7 +7,7 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np, torch
 import oracle
 from gpu_util import GL, ctx, dev, host, msm_inputs
-from ronkathon_b200 import ops, kzg, Polynomial, PlutoBaseField, PlutoScalarField
+from ronkathon_b200 import ops, kzg, curve, Polynomial, PlutoBaseField, PlutoScalarField
 
 c = ctx()
 ok = True
@@ -29,5 +29,9 @@ ok &= Polynomial([1, 2, 3, 4], PlutoBaseField).dft().evaluate(PlutoBaseField(2))
 pts, sc = msm_inputs(5000)
 ok &= ops.msm(c, torch.from_numpy(pts).cuda(), torch.from_numpy(sc).cuda()) == oracle.commit(sc, pts, fast=True)
 g1, _ = kzg.setup(); ok &= kzg.commit([7, 16, 1, 11, 1], g1).raw == bytes([32, 0, 59, 0])
+g1, g2 = kzg.setup()
+cm, pf = kzg.commit([3, 2, 1], g1), kzg.open_([3, 2, 1], 5, g1)
+ok &= kzg.check_batch([cm] * 3, [pf] * 3, [5] * 3, [4, 10, 4], g1, g2) == [True, False, True]
+ok &= curve.pairing(curve.AffinePoint(bytes([9, 37, 19, 93])), curve.AffinePoint(bytes([63, 0, 0, 35]))) == (26, 97)
 print("sanitize_smoke", "OK" if ok else "MISMATCH")
 sys.exit(0 if ok else 1)
