@@ -5,6 +5,21 @@
 
 using namespace ronk;
 
+// The device is bound (ronk_ctx_destroy, ronk_ctx_create); the DevBuf members free the device memory after this body.
+ronk_ctx::~ronk_ctx() {
+  for (auto& r : prof_log) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
+  for (int i = 0; i < kSlots; i++) {
+    if (ev_h2d[i]) cudaEventDestroy(ev_h2d[i]);
+    if (ev_compute[i]) cudaEventDestroy(ev_compute[i]);
+    if (ev_d2h[i]) cudaEventDestroy(ev_d2h[i]);
+  }
+  if (copy_in) cudaStreamDestroy(copy_in);
+  if (copy_out) cudaStreamDestroy(copy_out);
+  for (auto& b : scratch.blocks) cudaFreeAsync(b.base, stream);
+  cudaStreamSynchronize(stream);
+  if (h_flag) cudaFreeHost(h_flag);
+}
+
 extern "C" {
 
 const char* ronk_strerror(int code) {
@@ -71,11 +86,8 @@ int ronk_ctx_create(ronk_ctx** out, int device, void* stream) {
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete ctx; return RONK_ECUDA; }
   ctx->sm_count = prop.multiProcessorCount;
-  if (prop.major != 9 || prop.minor != 0) {  // sm_90a-only binary: loads on compute capability 9.0 alone
-    delete ctx;
-    return RONK_EUNSUPPORTED;
-  }
-  if (cudaMalloc((void**)&ctx->d_flag, sizeof(int)) != cudaSuccess ||
+  if (prop.major != 9 || prop.minor != 0) { delete ctx; return RONK_EUNSUPPORTED; }  // sm_90a-only binary: compute capability 9.0 alone
+  if (ctx->d_flag.alloc(ctx, 1) != RONK_OK ||
       cudaHostAlloc((void**)&ctx->h_flag, 32 * sizeof(int), cudaHostAllocMapped) != cudaSuccess) {  // h_flag[0] + 31 words of small results
     delete ctx;
     return RONK_ENOMEM;
@@ -89,44 +101,10 @@ int ronk_ctx_destroy(ronk_ctx* ctx) {
   ronk::DeviceGuard _dg(ctx);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->dist) ronk_dist_finalize(ctx);
-  for (auto& kv : ctx->plans) {
-    NttPlan& p = kv.second;
-    if (p.tw1) cudaFree(p.tw1);
-    if (p.tw2) cudaFree(p.tw2);
-    for (int d = 0; d < 2; d++) {
-      if (p.tw1_2d[d]) cudaFree(p.tw1_2d[d]);
-      if (p.tw2_2d[d]) cudaFree(p.tw2_2d[d]);
-    }
-    if (p.tw_lo) cudaFree(p.tw_lo);
-    if (p.tw_hi_inv) cudaFree(p.tw_hi_inv);
-    for (int d = 0; d < 2; d++) {
-      for (auto& t : p.tw_full[d]) cudaFree(t.second);
-      if (p.tw256[d]) cudaFree(p.tw256[d]);
-      if (p.t2[d]) cudaFree(p.t2[d]);
-      if (p.t1[d]) cudaFree(p.t1[d]);
-    }
-  }
-  for (auto& kv : ctx->anyntt_spec) cudaFree(kv.second);
-  for (auto& r : ctx->prof_log) { cudaEventDestroy(r.start); cudaEventDestroy(r.stop); }
-  for (int i = 0; i < ronk_ctx::kSlots; i++) {
-    if (ctx->slot_buf[i]) cudaFree(ctx->slot_buf[i]);
-    if (ctx->ev_h2d[i]) cudaEventDestroy(ctx->ev_h2d[i]);
-    if (ctx->ev_compute[i]) cudaEventDestroy(ctx->ev_compute[i]);
-    if (ctx->ev_d2h[i]) cudaEventDestroy(ctx->ev_d2h[i]);
-  }
-  if (ctx->copy_in) cudaStreamDestroy(ctx->copy_in);
-  if (ctx->copy_out) cudaStreamDestroy(ctx->copy_out);
-  for (auto& b : ctx->scratch.blocks) cudaFreeAsync(b.base, ctx->stream);
-  cudaStreamSynchronize(ctx->stream);
-  if (ctx->msm_ytab) cudaFree(ctx->msm_ytab);
-  if (ctx->msm_done) cudaFree(ctx->msm_done);
-  if (ctx->msm_coord) cudaFree(ctx->msm_coord);
-  if (ctx->pairing_tab) cudaFree(ctx->pairing_tab);
-  if (ctx->d_flag) cudaFree(ctx->d_flag);
-  if (ctx->h_flag) cudaFreeHost(ctx->h_flag);
   delete ctx;
   return RONK_OK;
 }
+
 
 int ronk_ctx_set_stream(ronk_ctx* ctx, void* stream) {
   ronk::DeviceGuard _dg(ctx);

@@ -111,12 +111,11 @@ struct DistState {
   u64* peer_ptr[16] = {};
   bool peer_opened[16] = {};
   // staging of the NCCL flavour
-  u64* pack = nullptr;
-  u64* recv = nullptr;
+  DevBuf<u64> pack, recv;
   size_t stage_words = 0;
-  int* barrier_word = nullptr;   // 4 bytes for the stream-ordered barrier
-  u32* gather = nullptr;         // G words for the commit all-gather (+1 for the local word)
-  std::map<std::tuple<u64, u64, u32>, u64*> twcol;  // (p, g, log_n) → ω_n^(rank·k'), k' < n/G
+  DevBuf<int> barrier_word;      // 4 bytes for the stream-ordered barrier
+  DevBuf<u32> gather;            // G words for the commit all-gather (+1 for the local word)
+  std::map<std::tuple<u64, u64, u32>, DevBuf<u64>> twcol;  // (p, g, log_n) → ω_n^(rank·k'), k' < n/G
 };
 
 struct PeerPtrs {
@@ -178,7 +177,7 @@ static int dist_check(ronk_ctx* ctx, DistState** out) {
 
 // stream-ordered barrier across the ranks: a 4-byte all-reduce on the context's stream
 static int dist_barrier(ronk_ctx* ctx, DistState* d) {
-  RONK_NCCL(ctx, nccl_api().AllReduce(d->barrier_word, d->barrier_word, 1, ncclInt32, ncclSum, d->comm, ctx->stream));
+  RONK_NCCL(ctx, nccl_api().AllReduce(d->barrier_word.get(), d->barrier_word.get(), 1, ncclInt32, ncclSum, d->comm, ctx->stream));
   return RONK_OK;
 }
 
@@ -187,9 +186,9 @@ static int dist_setup_common(ronk_ctx* ctx, DistState* d) {
     return set_err(ctx, RONK_EUNSUPPORTED, "world size must be a power of two ≤ 16");
   d->log_g = 0;
   while ((1 << d->log_g) < d->world) d->log_g++;
-  RONK_CUDA(ctx, cudaMalloc((void**)&d->barrier_word, sizeof(int)));
-  RONK_CUDA(ctx, cudaMemsetAsync(d->barrier_word, 0, sizeof(int), ctx->stream));
-  RONK_CUDA(ctx, cudaMalloc((void**)&d->gather, 17 * sizeof(u32)));
+  RONK_TRY(d->barrier_word.alloc(ctx, 1));
+  RONK_CUDA(ctx, cudaMemsetAsync(d->barrier_word.get(), 0, sizeof(int), ctx->stream));
+  RONK_TRY(d->gather.alloc(ctx, 17));
   return RONK_OK;
 }
 
@@ -219,14 +218,15 @@ static int dist_ensure_xbuf(ronk_ctx* ctx, DistState* d, size_t words) {
   mine.ptr = (unsigned long long)(uintptr_t)d->xbuf;
   mine.pid = (long long)getpid();
   mine.device = ctx->device;
-  PeerBuf* d_all = nullptr;
-  RONK_CUDA(ctx, cudaMalloc((void**)&d_all, sizeof(PeerBuf) * (size_t)(d->world + 1)));
-  RONK_CUDA(ctx, cudaMemcpyAsync(d_all + d->world, &mine, sizeof(mine), cudaMemcpyHostToDevice, ctx->stream));
-  RONK_NCCL(ctx, nccl_api().AllGather(d_all + d->world, d_all, sizeof(PeerBuf), ncclUint8, d->comm, ctx->stream));
+  DevBuf<PeerBuf> d_all;
+  RONK_TRY(d_all.alloc(ctx, (size_t)d->world + 1));
+  RONK_CUDA(ctx, cudaMemcpyAsync(d_all.get() + d->world, &mine, sizeof(mine), cudaMemcpyHostToDevice, ctx->stream));
+  RONK_NCCL(ctx, nccl_api().AllGather(d_all.get() + d->world, d_all.get(), sizeof(PeerBuf), ncclUint8, d->comm, ctx->stream));
   std::vector<PeerBuf> all((size_t)d->world);
-  RONK_CUDA(ctx, cudaMemcpyAsync(all.data(), d_all, sizeof(PeerBuf) * (size_t)d->world, cudaMemcpyDeviceToHost, ctx->stream));
+  RONK_CUDA(ctx, cudaMemcpyAsync(all.data(), d_all.get(), sizeof(PeerBuf) * (size_t)d->world, cudaMemcpyDeviceToHost,
+                                 ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  cudaFree(d_all);
+  d_all.reset();
   for (int r = 0; r < d->world; r++) {
     if (r == d->rank) { d->peer_ptr[r] = d->xbuf; continue; }
     if (all[(size_t)r].pid == mine.pid) {
@@ -252,30 +252,24 @@ static int dist_ensure_xbuf(ronk_ctx* ctx, DistState* d, size_t words) {
 static int dist_ensure_stage(ronk_ctx* ctx, DistState* d, size_t words) {
   if (d->stage_words >= words) return RONK_OK;
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (d->pack) cudaFree(d->pack);
-  if (d->recv) cudaFree(d->recv);
-  d->pack = d->recv = nullptr;
+  d->pack.reset();
+  d->recv.reset();
   d->stage_words = 0;
-  RONK_CUDA(ctx, cudaMalloc((void**)&d->pack, words * sizeof(u64)));
-  RONK_CUDA(ctx, cudaMalloc((void**)&d->recv, words * sizeof(u64)));
+  RONK_TRY(d->pack.alloc(ctx, words));
+  RONK_TRY(d->recv.alloc(ctx, words));
   d->stage_words = words;
   return RONK_OK;
 }
 
 // twiddle column ω_n^(rank·k'), k' < m, in the multiplier form f.mul expects (plain residues)
 static int dist_twcol(ronk_ctx* ctx, DistState* d, u64 p, u64 g, u32 log_n, const u64** out) {
-  auto key = std::make_tuple(p, g, log_n);
-  auto it = d->twcol.find(key);
-  if (it == d->twcol.end()) {
-    const size_t m = ((size_t)1 << log_n) >> d->log_g;
-    u64* tab = nullptr;
-    RONK_CUDA(ctx, cudaMalloc((void**)&tab, m * sizeof(u64)));
+  DevBuf<u64>& tab = d->twcol[std::make_tuple(p, g, log_n)];  // empty until built
+  const size_t m = ((size_t)1 << log_n) >> d->log_g;
+  if (!tab) RONK_TRY(build_table(ctx, &tab, m, [&](u64* t) {
     const u64 w = h_powmod(g, (p - 1) >> log_n, p);
-    const int rc = ronk_field_powers_u64(ctx, p, h_powmod(w, (u64)d->rank, p), 1 % p, (uint64_t*)tab, m);
-    if (rc != RONK_OK) { cudaFree(tab); return rc; }
-    it = d->twcol.emplace(key, tab).first;
-  }
-  *out = it->second;
+    return ronk_field_powers_u64(ctx, p, h_powmod(w, (u64)d->rank, p), 1 % p, t, m);
+  }));
+  *out = tab.get();
   return RONK_OK;
 }
 
@@ -316,11 +310,8 @@ static int dist_attach(ronk_ctx* ctx, ncclComm_t comm, bool owns, int rank, int 
   d->world = world;
   ctx->dist = d;
   const int rc = dist_setup_common(ctx, d);
-  if (rc != RONK_OK) {
-    ronk_dist_finalize(ctx);
-    return rc;
-  }
-  return RONK_OK;
+  if (rc != RONK_OK) ronk_dist_finalize(ctx);
+  return rc;
 }
 
 int ronk_dist_init(ronk_ctx* ctx, const uint8_t id[RONK_NCCL_UNIQUE_ID_BYTES], int rank, int world) {
@@ -355,11 +346,6 @@ int ronk_dist_finalize(ronk_ctx* ctx) {
   if (!d) return RONK_OK;
   cudaStreamSynchronize(ctx->stream);
   dist_release_xbuf(d);
-  if (d->pack) cudaFree(d->pack);
-  if (d->recv) cudaFree(d->recv);
-  if (d->barrier_word) cudaFree(d->barrier_word);
-  if (d->gather) cudaFree(d->gather);
-  for (auto& kv : d->twcol) cudaFree(kv.second);
   if (d->comm && d->owns_comm && nccl_api().ok) nccl_api().CommDestroy(d->comm);
   delete d;
   ctx->dist = nullptr;
@@ -440,18 +426,18 @@ int ronk_ntt_u64_dist(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* local, ui
   RONK_TRY(ntt_device_shared_mul(ctx, p, g, (const u64*)local, (u64*)local, twcol, log_m, batch));
   const u64* sendbase = (const u64*)local;
   if (batch > 1) {  // the block for destination s is strided over the batch: make it contiguous first
-    RONK_TRY(launch(ctx, "dist_pack", pack_blocks_kernel, grid_for(ctx, words, 256, 16), 256, 0, false, (const u64*)local, d->pack,
-                    blk, lg, batch));
-    sendbase = d->pack;
+    RONK_TRY(launch(ctx, "dist_pack", pack_blocks_kernel, grid_for(ctx, words, 256, 16), 256, 0, false, (const u64*)local,
+                    d->pack.get(), blk, lg, batch));
+    sendbase = d->pack.get();
   }
   const size_t chunk = (size_t)batch * blk;  // words per (source, destination) pair
   RONK_NCCL(ctx, n.GroupStart());
   for (int r = 0; r < G; r++) {
     RONK_NCCL(ctx, n.Send(sendbase + (size_t)r * chunk, chunk, ncclUint64, r, d->comm, ctx->stream));
-    RONK_NCCL(ctx, n.Recv(d->recv + (size_t)r * chunk, chunk, ncclUint64, r, d->comm, ctx->stream));
+    RONK_NCCL(ctx, n.Recv(d->recv.get() + (size_t)r * chunk, chunk, ncclUint64, r, d->comm, ctx->stream));
   }
   RONK_NCCL(ctx, n.GroupEnd());
-  for (int r = 0; r < G; r++) src.p[r] = d->recv + (size_t)r * chunk;
+  for (int r = 0; r < G; r++) src.p[r] = d->recv.get() + (size_t)r * chunk;
   return cross_rank(ctx, p, g, lg, src, (u64*)local, blk, batch, blk, 0, m);
 }
 
@@ -478,34 +464,31 @@ int ronk_ntt_u64_dist_virtual(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* d
   const u32 log_m = log_n - log_g;
   const int G = 1 << log_g;
   const size_t m = (size_t)1 << log_m, blk = m >> log_g, words = (size_t)batch * m, chunk = (size_t)batch * blk;
-  struct Scratch {
-    u64 *z = nullptr, *tw = nullptr, *pack = nullptr;
-    ~Scratch() { if (z) cudaFree(z); if (tw) cudaFree(tw); if (pack) cudaFree(pack); }
-  } sc;
-  RONK_CUDA(ctx, cudaMalloc((void**)&sc.z, (size_t)G * words * sizeof(u64)));   // FUSED: the G exchange buffers; NCCL: the G receive buffers
-  RONK_CUDA(ctx, cudaMalloc((void**)&sc.tw, m * sizeof(u64)));
-  if (flavour == RONK_DIST_NCCL) RONK_CUDA(ctx, cudaMalloc((void**)&sc.pack, words * sizeof(u64)));
+  DevBuf<u64> z, tw, pack;
+  RONK_TRY(z.alloc(ctx, (size_t)G * words));   // FUSED: the G exchange buffers; NCCL: the G receive buffers
+  RONK_TRY(tw.alloc(ctx, m));
+  if (flavour == RONK_DIST_NCCL) RONK_TRY(pack.alloc(ctx, words));
   const u64 w = h_powmod(g, (p - 1) >> log_n, p);
   for (int r = 0; r < G; r++) {   // Z_r = NTT_m(a[r::G]) ⊙ ω_n^(r·k')
     u64* local = (u64*)data + (size_t)r * words;
     const u64* twcol = nullptr;
     if (r) {
-      RONK_TRY(ronk_field_powers_u64(ctx, p, h_powmod(w, (u64)r, p), 1 % p, (uint64_t*)sc.tw, m));
-      twcol = sc.tw;
+      RONK_TRY(ronk_field_powers_u64(ctx, p, h_powmod(w, (u64)r, p), 1 % p, tw.get(), m));
+      twcol = tw.get();
     }
     if (flavour == RONK_DIST_FUSED) {
-      RONK_TRY(ntt_device_shared_mul(ctx, p, g, local, sc.z + (size_t)r * words, twcol, log_m, batch));
+      RONK_TRY(ntt_device_shared_mul(ctx, p, g, local, z.get() + (size_t)r * words, twcol, log_m, batch));
     } else {
       RONK_TRY(ntt_device_shared_mul(ctx, p, g, local, local, twcol, log_m, batch));
       const u64* sendbase = local;
       if (batch > 1) {
-        RONK_TRY(launch(ctx, "dist_pack", pack_blocks_kernel, grid_for(ctx, words, 256, 16), 256, 0, false, local, sc.pack, blk,
+        RONK_TRY(launch(ctx, "dist_pack", pack_blocks_kernel, grid_for(ctx, words, 256, 16), 256, 0, false, local, pack.get(), blk,
                         log_g, batch));
-        sendbase = sc.pack;
+        sendbase = pack.get();
       }
       // the all-to-all: source r's chunk for destination s lands in s's receive buffer at slot r
       for (int s2 = 0; s2 < G; s2++)
-        RONK_CUDA(ctx, cudaMemcpyAsync(sc.z + (size_t)s2 * words + (size_t)r * chunk, sendbase + (size_t)s2 * chunk,
+        RONK_CUDA(ctx, cudaMemcpyAsync(z.get() + (size_t)s2 * words + (size_t)r * chunk, sendbase + (size_t)s2 * chunk,
                                        chunk * sizeof(u64), cudaMemcpyDeviceToDevice, ctx->stream));
     }
   }
@@ -514,10 +497,10 @@ int ronk_ntt_u64_dist_virtual(ronk_ctx* ctx, uint64_t p, uint64_t g, uint64_t* d
     for (int q = 0; q < 16; q++) src.p[q] = nullptr;
     u64* local = (u64*)data + (size_t)r * words;
     if (flavour == RONK_DIST_FUSED) {
-      for (int q = 0; q < G; q++) src.p[q] = sc.z + (size_t)q * words;
+      for (int q = 0; q < G; q++) src.p[q] = z.get() + (size_t)q * words;
       RONK_TRY(cross_rank(ctx, p, g, log_g, src, local, blk, batch, m, (size_t)r * blk, m));
     } else {
-      for (int q = 0; q < G; q++) src.p[q] = sc.z + (size_t)r * words + (size_t)q * chunk;
+      for (int q = 0; q < G; q++) src.p[q] = z.get() + (size_t)r * words + (size_t)q * chunk;
       RONK_TRY(cross_rank(ctx, p, g, log_g, src, local, blk, batch, blk, 0, m));
     }
   }
@@ -536,10 +519,11 @@ int ronk_msm_pluto_ext_dist(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   // every rank takes part in the collective even if its shard was rejected (the flag travels with the point)
   u32 word = (rc_local == RONK_OK) ? ((u32)mine[0] | ((u32)mine[1] << 8) | ((u32)mine[2] << 16) | ((u32)mine[3] << 24))
                                    : 0xFFFFFFFEu;  // not a valid packing: marks a failed shard
-  RONK_CUDA(ctx, cudaMemcpyAsync(d->gather + 16, &word, sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
-  RONK_NCCL(ctx, nccl_api().AllGather(d->gather + 16, d->gather, 1, ncclUint32, d->comm, ctx->stream));
+  u32* gather = d->gather.get();
+  RONK_CUDA(ctx, cudaMemcpyAsync(gather + 16, &word, sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
+  RONK_NCCL(ctx, nccl_api().AllGather(gather + 16, gather, 1, ncclUint32, d->comm, ctx->stream));
   u32 all[16];
-  RONK_CUDA(ctx, cudaMemcpyAsync(all, d->gather, sizeof(u32) * (size_t)d->world, cudaMemcpyDeviceToHost, ctx->stream));
+  RONK_CUDA(ctx, cudaMemcpyAsync(all, gather, sizeof(u32) * (size_t)d->world, cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   for (int r = 0; r < d->world; r++)
     if (all[r] == 0xFFFFFFFEu)
@@ -548,7 +532,7 @@ int ronk_msm_pluto_ext_dist(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   u32* host_dev = nullptr;
   RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&host_dev, (void*)ctx->h_flag, 0));
   host[1] = PT_INF;
-  RONK_TRY(launch(ctx, "point_sum", point_sum_kernel, 1, 32, 0, false, d->gather, (u32)d->world, host_dev + 1));
+  RONK_TRY(launch(ctx, "point_sum", point_sum_kernel, 1, 32, 0, false, gather, (u32)d->world, host_dev + 1));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   const u32 res = host[1];
   out[0] = (uint8_t)(res & 0xFF);

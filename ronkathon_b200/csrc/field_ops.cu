@@ -149,7 +149,7 @@ static int binop(ronk_ctx* ctx, u64 p, const u64* a, const u64* b, u64* out, siz
   if (OP == OP_DIV) RONK_TRY(reset_flag(ctx));
   RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
     return launch(ctx, name, binop_kernel<std::decay_t<decltype(f)>, OP>, grid_for(ctx, n, 256), 256, 0, false, f, a, b,
-                  out, n, ctx->d_flag);
+                  out, n, ctx->d_flag.get());
   }));
   if (OP == OP_DIV) {
     int v = 0;
@@ -167,7 +167,7 @@ static int unop(ronk_ctx* ctx, u64 p, const u64* a, u64* out, size_t n, u64 e, c
   if (OP == UOP_INV) RONK_TRY(reset_flag(ctx));
   RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
     return launch(ctx, name, unop_kernel<std::decay_t<decltype(f)>, OP>, grid_for(ctx, n, 256), 256, 0, false, f, a, out,
-                  n, e, ctx->d_flag);
+                  n, e, ctx->d_flag.get());
   }));
   if (OP == UOP_INV) {
     int v = 0;

@@ -417,10 +417,11 @@ int msm_coord_tables(ronk_ctx* ctx) {
   std::vector<u32> tabs(kTabWords + MSM_EXP * MSM_EXP + 4, 0xFFFFFFFFu);
   if (!build_group_tables(tabs.data(), tabs.data() + kTabWords)) return set_err(ctx, RONK_ECUDA, "internal: no basis of E(F_101^2) found");
   tabs[kTabWords + MSM_EXP * MSM_EXP + 0] = tabs[kTabWords + MSM_EXP * MSM_EXP + 1] = tabs[kTabWords + MSM_EXP * MSM_EXP + 2] = 0u;
-  RONK_CUDA(ctx, cudaMalloc(&ctx->msm_coord, tabs.size() * sizeof(u32)));
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->msm_coord, tabs.data(), tabs.size() * sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
-  RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // tabs is pageable and goes out of scope
-  return RONK_OK;
+  return build_table(ctx, &ctx->msm_coord, tabs.size(), [&](u32* tab) {
+    RONK_CUDA(ctx, cudaMemcpyAsync(tab, tabs.data(), tabs.size() * sizeof(u32), cudaMemcpyHostToDevice, ctx->stream));
+    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // tabs is pageable and goes out of scope
+    return RONK_OK;
+  });
 }
 
 static int msm_coord_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points, const uint8_t* scalars, size_t n_scalars,
@@ -432,10 +433,10 @@ static int msm_coord_device(ronk_ctx* ctx, const uint8_t* points, size_t n_point
   constexpr size_t kSmem = kTabWords * sizeof(u32);
   RONK_TRY(msm_coord_tables(ctx));
   RONK_TRY(ensure_smem_attr(ctx, msm_coord_kernel, (int)kSmem));
-  const u32* bintab = (const u32*)ctx->msm_coord;
+  const u32* bintab = ctx->msm_coord.get();
   const u32* pttab = bintab + kTabWords;
   static_assert((kTabWords + MSM_EXP * MSM_EXP) % 2 == 0, "the 64-bit accumulator must be 8-byte aligned");
-  unsigned long long* gacc = (unsigned long long*)((u32*)ctx->msm_coord + kTabWords + MSM_EXP * MSM_EXP);
+  unsigned long long* gacc = (unsigned long long*)(ctx->msm_coord.get() + kTabWords + MSM_EXP * MSM_EXP);
   // a CTA is worth its 82 KB table load once every thread sees ≥ 4 terms
   const int ctas = grid_for(ctx, n_scalars, MSM_COORD_THREADS * 4, 1);
   const int vec = (((uintptr_t)points & 15) == 0 && ((uintptr_t)scalars & 3) == 0) ? 1 : 0;
@@ -605,7 +606,7 @@ static int msm_batch_device(ronk_ctx* ctx, const uint8_t* points, size_t n_point
     return RONK_OK;
   }
   RONK_TRY(msm_coord_tables(ctx));
-  const u32* bintab = (const u32*)ctx->msm_coord;
+  const u32* bintab = ctx->msm_coord.get();
   const u32* pttab = bintab + kTabWords;
   const size_t plane_words = (n_scalars + 15) / 16 * 4;   // each plane: ⌈n/16⌉·16 bytes
   const u64 cols = ((n_scalars + 3) / 4 + MSM_ROWS_CHUNK - 1) / MSM_ROWS_CHUNK;
@@ -667,20 +668,25 @@ static int msm_hist_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points
   if (n_scalars == 0) { *h_result = PT_INF; return RONK_OK; }   // empty sum = Infinity (curve/mod.rs:219-223)
   constexpr size_t kSmem = MSM_BINS * sizeof(u32) + MSM_BINS * sizeof(uint16_t);
   if (!ctx->msm_ytab) {  // one-time per context: curve tables, completion counter
-    uint16_t* sq = nullptr;
-    RONK_CUDA(ctx, cudaMalloc((void**)&sq, MSM_XS * sizeof(uint16_t)));
-    RONK_CUDA(ctx, cudaMalloc((void**)&ctx->msm_ytab, MSM_BINS * sizeof(uint16_t)));
-    RONK_CUDA(ctx, cudaMalloc((void**)&ctx->msm_done, (1 + MSM_BINS) * sizeof(u32)));  // counter + global histogram
-    RONK_CUDA(ctx, cudaMemsetAsync(sq, 0xFF, MSM_XS * sizeof(uint16_t), ctx->stream));
-    RONK_CUDA(ctx, cudaMemsetAsync(ctx->msm_done, 0, (1 + MSM_BINS) * sizeof(u32), ctx->stream));
-    {
-      LaunchScope ls(ctx, "msm_tables");
-      msm_sqrt_table_kernel<<<(MSM_XS + 255) / 256, 256, 0, ctx->stream>>>(sq);
-      msm_ytab_kernel<<<(MSM_XS + 255) / 256, 256, 0, ctx->stream>>>(sq, (uint16_t*)ctx->msm_ytab);
-    }
-    RONK_TRY(check_launch(ctx, "msm table kernels"));
-    RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    cudaFree(sq);
+    DevBuf<uint16_t> sq, ytab;
+    DevBuf<u32> done;
+    RONK_TRY(build_tables(ctx, [&] {
+      RONK_TRY(sq.alloc(ctx, MSM_XS));
+      RONK_TRY(ytab.alloc(ctx, MSM_BINS));
+      RONK_TRY(done.alloc(ctx, 1 + MSM_BINS));  // counter + global histogram
+      RONK_CUDA(ctx, cudaMemsetAsync(sq.get(), 0xFF, MSM_XS * sizeof(uint16_t), ctx->stream));
+      RONK_CUDA(ctx, cudaMemsetAsync(done.get(), 0, (1 + MSM_BINS) * sizeof(u32), ctx->stream));
+      {
+        LaunchScope ls(ctx, "msm_tables");
+        msm_sqrt_table_kernel<<<(MSM_XS + 255) / 256, 256, 0, ctx->stream>>>(sq.get());
+        msm_ytab_kernel<<<(MSM_XS + 255) / 256, 256, 0, ctx->stream>>>(sq.get(), ytab.get());
+      }
+      RONK_TRY(check_launch(ctx, "msm table kernels"));
+      RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      return RONK_OK;
+    }));
+    ctx->msm_ytab = std::move(ytab);
+    ctx->msm_done = std::move(done);
   }
   RONK_TRY(ensure_smem_attr(ctx, msm_hist_kernel, (int)kSmem));
   // one CTA per SM at most; each thread should see ≥ 8 terms before another CTA (its table load and its 82 KB of
@@ -693,16 +699,16 @@ static int msm_hist_device(ronk_ctx* ctx, const uint8_t* points, size_t n_points
   RONK_TRY(fr.take(&partial, ctas * MSM_BINS + fin_ctas));
   u32* cta_sum = partial + ctas * MSM_BINS;
   // the split between shared-memory and L2 atomics pays once the SM's atomic unit is the limiter
-  u32* ghist = (n_scalars >= ((size_t)1 << 22) && ctx->tune.msm_split) ? (u32*)ctx->msm_done + 1 : nullptr;
+  u32* ghist = (n_scalars >= ((size_t)1 << 22) && ctx->tune.msm_split) ? ctx->msm_done.get() + 1 : nullptr;
   volatile u32* host = (volatile u32*)ctx->h_flag;  // mapped pinned: [0] = flag, [1] = result
   host[0] = 0u;
   host[1] = PT_INF;
   u32* host_dev = nullptr;
   RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&host_dev, (void*)ctx->h_flag, 0));
   RONK_TRY(launch(ctx, "msm_hist", msm_hist_kernel, (unsigned)ctas, MSM_HIST_THREADS, kSmem, false, (const u32*)points, scalars,
-                  n_scalars, (const uint16_t*)ctx->msm_ytab, partial, ghist, (volatile int*)host_dev));
+                  n_scalars, (const uint16_t*)ctx->msm_ytab.get(), partial, ghist, (volatile int*)host_dev));
   RONK_TRY(launch(ctx, "msm_hist_finish", msm_hist_finish_kernel, fin_ctas, MSM_FIN_THREADS * MSM_FIN_GROUPS, 0, ctx->tune.pdl,
-                  partial, (u32)ctas, ghist, (const uint16_t*)ctx->msm_ytab, cta_sum, (u32*)ctx->msm_done, host_dev + 1));
+                  partial, (u32)ctas, ghist, (const uint16_t*)ctx->msm_ytab.get(), cta_sum, ctx->msm_done.get(), host_dev + 1));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (host[0]) return set_err(ctx, RONK_EINVAL, "off-curve point, non-canonical coordinate or scalar >= 17");
   *h_result = host[1];
@@ -834,7 +840,7 @@ static int point_op_host(ronk_ctx* ctx, int op, const uint8_t* a, const uint8_t*
   RONK_TRY(stage_in(fr, s));
   RONK_TRY(reset_flag(ctx));
   RONK_TRY(launch(ctx, "point_op", point_op_kernel, grid_for(ctx, n, 128), 128, 0, false, op, (const u32*)s[0].dev,
-                  (const u32*)s[1].dev, (const uint8_t*)s[2].dev, (u32*)s[3].dev, n, ctx->d_flag));
+                  (const u32*)s[1].dev, (const uint8_t*)s[2].dev, (u32*)s[3].dev, n, ctx->d_flag.get()));
   int v = 0;
   RONK_TRY(read_flag(ctx, &v));
   if (v) return set_err(ctx, RONK_EINVAL, "Point is not on curve / scalar out of range");

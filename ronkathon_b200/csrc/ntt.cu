@@ -32,18 +32,18 @@ int make_mont_field(ronk_ctx* ctx, u64 p, u64 g, bool inverse, MontField* out) {
 }
 
 template <class F>
-static int build_table(ronk_ctx* ctx, const F& f, u64 w, u64 s, u64** tab, u32 count) {
-  RONK_CUDA(ctx, cudaMalloc((void**)tab, (size_t)count * sizeof(u64)));
-  return launch(ctx, "pow_table", pow_table_kernel<F>, (count + 255) / 256, 256, 0, false, f, w, s, *tab, count);
+static int build_pow_table(ronk_ctx* ctx, const F& f, u64 w, u64 s, DevBuf<u64>* tab, u32 count) {
+  RONK_TRY(tab->alloc(ctx, count));
+  return launch(ctx, "pow_table", pow_table_kernel<F>, (count + 255) / 256, 256, 0, false, f, w, s, tab->get(), count);
 }
 
-static int build_tw2d(ronk_ctx* ctx, const u64* tw1d, u32 log_m, u64* out2d[2]) {
+static int build_tw2d(ronk_ctx* ctx, const u64* tw1d, u32 log_m, DevBuf<u64> out2d[2]) {
   u32 off[4];
   const u32 words = ntt_tw2d_layout(log_m, off);
   for (int d = 0; d < 2; d++) {
-    RONK_CUDA(ctx, cudaMalloc((void**)&out2d[d], (size_t)(words ? words : 2) * sizeof(u64)));
+    RONK_TRY(out2d[d].alloc(ctx, words ? words : 2));
     if (!words) continue;
-    RONK_TRY(launch(ctx, "tw2d_gather", tw2d_gather_kernel, (words + 255) / 256, 256, 0, false, tw1d, log_m, d, out2d[d], words));
+    RONK_TRY(launch(ctx, "tw2d_gather", tw2d_gather_kernel, (words + 255) / 256, 256, 0, false, tw1d, log_m, d, out2d[d].get(), words));
   }
   return RONK_OK;
 }
@@ -59,19 +59,19 @@ static int build_plan(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, NttPla
   const NttShape sh = ntt_shape(log_n);
   if (!sh.two_pass) {
     plan->two_pass = false;
-    RONK_TRY(build_table(ctx, f, w, 1, &plan->tw1, (u32)n));
-    RONK_TRY(build_tw2d(ctx, plan->tw1, log_n, plan->tw1_2d));
+    RONK_TRY(build_pow_table(ctx, f, w, 1, &plan->tw1, (u32)n));
+    RONK_TRY(build_tw2d(ctx, plan->tw1.get(), log_n, plan->tw1_2d));
   } else {
     plan->two_pass = true;
     plan->log_n1 = sh.log_n1;
     plan->log_n2 = sh.log_n2;
     const u64 n1 = (u64)1 << plan->log_n1, n2 = (u64)1 << plan->log_n2;
-    RONK_TRY(build_table(ctx, f, h_powmod(w, n2, p), 1, &plan->tw1, (u32)n1));
-    RONK_TRY(build_table(ctx, f, h_powmod(w, n1, p), 1, &plan->tw2, (u32)n2));
-    RONK_TRY(build_table(ctx, f, w, 1, &plan->tw_lo, (u32)n1));
-    RONK_TRY(build_table(ctx, f, h_powmod(w, n1, p), ninv, &plan->tw_hi_inv, (u32)n2));
-    RONK_TRY(build_tw2d(ctx, plan->tw1, plan->log_n1, plan->tw1_2d));
-    RONK_TRY(build_tw2d(ctx, plan->tw2, plan->log_n2, plan->tw2_2d));
+    RONK_TRY(build_pow_table(ctx, f, h_powmod(w, n2, p), 1, &plan->tw1, (u32)n1));
+    RONK_TRY(build_pow_table(ctx, f, h_powmod(w, n1, p), 1, &plan->tw2, (u32)n2));
+    RONK_TRY(build_pow_table(ctx, f, w, 1, &plan->tw_lo, (u32)n1));
+    RONK_TRY(build_pow_table(ctx, f, h_powmod(w, n1, p), ninv, &plan->tw_hi_inv, (u32)n2));
+    RONK_TRY(build_tw2d(ctx, plan->tw1.get(), plan->log_n1, plan->tw1_2d));
+    RONK_TRY(build_tw2d(ctx, plan->tw2.get(), plan->log_n2, plan->tw2_2d));
   }
   // n^-1 in twiddle form: Goldilocks → plain; Montgomery → ninv·R mod p
   if (p == GL_P && g == 7) plan->scale_inv = ninv;
@@ -80,25 +80,17 @@ static int build_plan(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, NttPla
 }
 
 // n-word table of the inter-pass twiddles for one direction and one workspace layout (log2 C2), built on first use.
-// The table pointer is cached in the plan.
+// The table is cached in the plan; *out = nullptr where there is no memory for it: the stepped form needs none.
 template <class F>
 static int interpass_table(ronk_ctx* ctx, const F& f, NttPlan& pl, bool inverse, u32 log_c2, const u64* tw_lo,
                            const u64* tw_hi, const u64** out) {
-  auto& m = pl.tw_full[inverse ? 1 : 0];
-  auto it = m.find(log_c2);
-  if (it == m.end()) {
-    u64* tab = nullptr;
-    const u64 n = (u64)1 << pl.log_n;
-    if (cudaMalloc((void**)&tab, n * sizeof(u64)) != cudaSuccess) {
-      cudaGetLastError();
-      *out = nullptr;  // no memory for the table: the stepped form needs none
-      return RONK_OK;
-    }
-    RONK_TRY(launch(ctx, "interpass_table", interpass_table_kernel<F>, (unsigned)((n + 255) / 256), 256, 0, false, f, tw_lo,
-                    tw_hi, pl.log_n, pl.log_n1, pl.log_n2, log_c2, pl.log_n1, inverse ? 1 : 0, tab));
-    it = m.emplace(log_c2, tab).first;
-  }
-  *out = it->second;
+  DevBuf<u64>& tab = pl.tw_full[inverse ? 1 : 0][log_c2];  // empty until built
+  const u64 n = (u64)1 << pl.log_n;
+  if (!tab) RONK_TRY(build_table(ctx, &tab, n, [&](u64* t) {
+    return launch(ctx, "interpass_table", interpass_table_kernel<F>, (unsigned)((n + 255) / 256), 256, 0, false, f, tw_lo, tw_hi,
+                  pl.log_n, pl.log_n1, pl.log_n2, log_c2, pl.log_n1, inverse ? 1 : 0, t);
+  }, true));
+  *out = tab.get();
   return RONK_OK;
 }
 
@@ -216,10 +208,16 @@ static int ntt3_tables(ronk_ctx* ctx, const F& f, NttPlan& pl, int log_n) {
   const u64 p = pl.p, n = (u64)1 << log_n;
   u64 w = h_powmod(pl.g, (p - 1) / n, p);
   if (INV) w = h_powmod(w, p - 2, p);
-  RONK_TRY(build_table(ctx, f, h_powmod(w, n >> 8, p), 1, &pl.tw256[d], 256));
-  RONK_CUDA(ctx, cudaMalloc((void**)&pl.t2[d], 65536 * sizeof(u64)));
-  const u64 ninv = INV ? h_powmod(n % p, p - 2, p) : 1;
-  return launch(ctx, "ntt3_t2", ntt3_t2_kernel<F>, 256, 256, 0, false, f, h_powmod(w, n >> 16, p), ninv, pl.t2[d]);
+  DevBuf<u64> tw256, t2;
+  RONK_TRY(build_tables(ctx, [&] {
+    RONK_TRY(build_pow_table(ctx, f, h_powmod(w, n >> 8, p), 1, &tw256, 256));
+    RONK_TRY(t2.alloc(ctx, 65536));
+    const u64 ninv = INV ? h_powmod(n % p, p - 2, p) : 1;
+    return launch(ctx, "ntt3_t2", ntt3_t2_kernel<F>, 256, 256, 0, false, f, h_powmod(w, n >> 16, p), ninv, t2.get());
+  }));
+  pl.tw256[d] = std::move(tw256);
+  pl.t2[d] = std::move(t2);
+  return RONK_OK;
 }
 
 // Small batches of 2^16-point transforms in ONE launch: a 16-CTA thread-block cluster per transform, the pass-2 → pass-3
@@ -244,8 +242,8 @@ static int run_ntt16_cluster(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, 
   }
   const int d = INV ? 1 : 0;
   Ntt3Args A = {};
-  A.tw256 = pl.tw256[d];
-  A.t2 = pl.t2[d];
+  A.tw256 = pl.tw256[d].get();
+  A.t2 = pl.t2[d].get();
   A.batch = batch;
   A.src_len = A.dst_len = NTT_UNBOUNDED;
   A.src = src;
@@ -301,24 +299,21 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
   RONK_TRY((ntt3_tables<F, INV>(ctx, f, pl, LOGN)));
   if (LOGN >= 20 && LOGN <= ctx->tune.ntt3_t1 && !pl.t1[d]) {  // n-word table of the stepped twiddles: 8 MiB (2^20) … 128 MiB (2^24) per direction; no memory: stay stepped
     if (pl.log_n1 != (u32)(LOGN + 1) / 2 || !pl.tw_lo || !pl.tw2) return set_err(ctx, RONK_ECUDA, "internal: unexpected plan shape");
-    if (cudaMalloc((void**)&pl.t1[d], n * sizeof(u64)) != cudaSuccess) {
-      cudaGetLastError();
-      pl.t1[d] = nullptr;
-    } else if (LOGN >= 21) {
-      RONK_TRY(launch(ctx, "ntt3_t1", ntt3_t1_kernel<F>, (unsigned)(n / 256), 256, 0, false, f, pl.tw_lo, pl.tw2, INV ? 1 : 0,
-                      pl.t1[d], (u32)LOGN));
-    } else {
-      RONK_TRY(launch(ctx, "ntt3_t1", ntt3_t1_20_kernel<F>, (unsigned)(n / 256), 256, 0, false, f, pl.tw_lo, pl.tw2, INV ? 1 : 0,
-                      pl.t1[d]));
-    }
+    RONK_TRY(build_table(ctx, &pl.t1[d], n, [&](u64* t1) {
+      if (LOGN >= 21)
+        return launch(ctx, "ntt3_t1", ntt3_t1_kernel<F>, (unsigned)(n / 256), 256, 0, false, f, pl.tw_lo.get(), pl.tw2.get(),
+                      INV ? 1 : 0, t1, (u32)LOGN);
+      return launch(ctx, "ntt3_t1", ntt3_t1_20_kernel<F>, (unsigned)(n / 256), 256, 0, false, f, pl.tw_lo.get(), pl.tw2.get(),
+                    INV ? 1 : 0, t1);
+    }, true));
   }
   if (LI > 0) {
     if (!outer || !outer->tw_lo || !outer->tw2 || batch > (0x7FFFFFFFu >> (12 + LI))) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
     Ntt3Args P = {};
     P.src = src;
     P.dst = data;
-    P.tw_lo = outer->tw_lo;
-    P.tw_hi = outer->tw2;
+    P.tw_lo = outer->tw_lo.get();
+    P.tw_hi = outer->tw2.get();
     P.scale_tw = INV ? f.to_tw(h_powmod((u64)1 << LI, pl.p - 2, pl.p)) : 0;   // 2^-LI: the rest of n^-1 rides on the sub-transforms' tables
     P.batch = batch;
     RONK_TRY((launch3p<F, INV, LI>(ctx, f, P, (u32)LOGN, outer->log_n1, INV ? "intt3_split" : "ntt3_split")));
@@ -331,11 +326,11 @@ static int run_ntt3(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64
   RONK_TRY(fr.take(&ws, (size_t)batch << LOGN));
   if (LOGN >= 20 && (pl.log_n1 != (u32)(LOGN + 1) / 2 || !pl.tw_lo || !pl.tw2)) return set_err(ctx, RONK_ECUDA, "internal: unexpected plan shape");
   Ntt3Args A = {};
-  A.t1 = LOGN <= ctx->tune.ntt3_t1 ? pl.t1[d] : nullptr;
-  A.tw256 = pl.tw256[d];
-  A.tw_lo = pl.tw_lo;
-  A.tw_hi = pl.tw2;   // ω_n^(4096 y), plain: the n^-1 of the inverse rides on the pass-2 table
-  A.t2 = pl.t2[d];
+  A.t1 = LOGN <= ctx->tune.ntt3_t1 ? pl.t1[d].get() : nullptr;
+  A.tw256 = pl.tw256[d].get();
+  A.tw_lo = pl.tw_lo.get();
+  A.tw_hi = pl.tw2.get();   // ω_n^(4096 y), plain: the n^-1 of the inverse rides on the pass-2 table
+  A.t2 = pl.t2[d].get();
   A.batch = batch;
   A.src_len = src_len;
   A.dst_len = dst_len;
@@ -380,8 +375,8 @@ static int plan_for(ronk_ctx* ctx, const F& f, u64 p, u64 g, u32 log_n, NttPlan*
   auto it = ctx->plans.find(key);
   if (it == ctx->plans.end()) {
     NttPlan pl;
-    RONK_TRY(build_plan(ctx, f, p, g, log_n, &pl));
-    it = ctx->plans.emplace(key, pl).first;
+    RONK_TRY(build_tables(ctx, [&] { return build_plan(ctx, f, p, g, log_n, &pl); }));
+    it = ctx->plans.emplace(key, std::move(pl)).first;
   }
   *out = &it->second;
   return RONK_OK;
@@ -407,7 +402,7 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
   if (!pl.two_pass) {
     const u32 cap = (u32)ctx->tune.single_tile_log;
     NttTileArgs A =
-        ntt_args_single(data, mul, pl.tw1_2d[INV ? 1 : 0], pl.scale_inv, log_n, (u64)batch << log_n, INV, cap, &tiles);
+        ntt_args_single(data, mul, pl.tw1_2d[INV ? 1 : 0].get(), pl.scale_inv, log_n, (u64)batch << log_n, INV, cap, &tiles);
     A.src = src;
     A.src_len = src_len;
     A.dst_len = dst_len;
@@ -487,8 +482,8 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
   u32 tile1, tile2;
   ntt_pass_tiles(log_n, p1, p2, &tile1, &tile2);
   // pass 1: N1-point transforms down the columns, inter-pass twiddle, blocked write to the workspace
-  NttTileArgs A1 = ntt_args_pass1(src, ws, pl.tw1_2d[INV ? 1 : 0], pl.tw_lo, INV ? pl.tw_hi_inv : pl.tw2, pl.tw2,
-                                  log_n, batch, tile1, tile2, &tiles);
+  NttTileArgs A1 = ntt_args_pass1(src, ws, pl.tw1_2d[INV ? 1 : 0].get(), pl.tw_lo.get(), (INV ? pl.tw_hi_inv : pl.tw2).get(),
+                                  pl.tw2.get(), log_n, batch, tile1, tile2, &tiles);
   A1.src_len = src_len;
   if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
   if (coset) {   // the hooked pass is the first (forward) or the last (inverse); launch_tile_n picks it
@@ -504,7 +499,7 @@ static int run_ntt(ronk_ctx* ctx, const F& f, NttPlan& pl, u64* data, const u64*
   const char* name1 = coset ? (INV ? "intt_pass1_coset" : "ntt_pass1_coset") : (INV ? "intt_pass1" : "ntt_pass1");
   RONK_TRY((launch_tile<F, MODE_PASS1, INV>(ctx, f, A1, (u32)tiles, name1)));
   // pass 2: N2-point transforms along the contiguous workspace tiles, natural-order output
-  NttTileArgs A2 = ntt_args_pass2(ws, data, mul, pl.tw2_2d[INV ? 1 : 0], log_n, batch, tile2, &tiles);
+  NttTileArgs A2 = ntt_args_pass2(ws, data, mul, pl.tw2_2d[INV ? 1 : 0].get(), log_n, batch, tile2, &tiles);
   A2.dst_len = dst_len;
   A2.mul_mask = mul_mask;
   if (tiles > 0x7FFFFFFFULL) return set_err(ctx, RONK_EUNSUPPORTED, "batch too large");
@@ -567,8 +562,8 @@ int ntt_single_tables(ronk_ctx* ctx, u64 p, u64 g, u32 log_n, const u64** fwd, c
   return with_field(ctx, p, g, false, [&](const auto& f) {
     NttPlan* pl = nullptr;
     RONK_TRY(plan_for(ctx, f, p, g, log_n, &pl));
-    *fwd = pl->tw1_2d[0];
-    *inv = pl->tw1_2d[1];
+    *fwd = pl->tw1_2d[0].get();
+    *inv = pl->tw1_2d[1].get();
     *scale_inv = pl->scale_inv;
     return RONK_OK;
   });
@@ -660,16 +655,12 @@ extern "C" int ronk_ntt_u64_host_submit(ronk_ctx* ctx, uint64_t p, uint64_t g, u
   RONK_TRY(pipeline_init(ctx));
   RONK_TRY(ronk_ntt_u64_host_wait(ctx, slot));  // the slot's previous occupant must be home first
   if (ctx->slot_bytes[slot] < bytes) {
-    if (ctx->slot_buf[slot]) {
-      RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      RONK_CUDA(ctx, cudaFree(ctx->slot_buf[slot]));
-      ctx->slot_buf[slot] = nullptr;
-      ctx->slot_bytes[slot] = 0;
-    }
-    RONK_CUDA(ctx, cudaMalloc(&ctx->slot_buf[slot], bytes));
+    if (ctx->slot_buf[slot]) RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // alloc frees the old buffer first
+    ctx->slot_bytes[slot] = 0;
+    RONK_TRY(ctx->slot_buf[slot].alloc(ctx, bytes / sizeof(u64)));
     ctx->slot_bytes[slot] = bytes;
   }
-  u64* dbuf = (u64*)ctx->slot_buf[slot];
+  u64* dbuf = ctx->slot_buf[slot].get();
   RONK_CUDA(ctx, cudaMemcpyAsync(dbuf, host_data, bytes, cudaMemcpyHostToDevice, ctx->copy_in));
   RONK_CUDA(ctx, cudaEventRecord(ctx->ev_h2d[slot], ctx->copy_in));
   RONK_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_h2d[slot], 0));

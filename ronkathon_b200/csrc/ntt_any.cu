@@ -145,29 +145,18 @@ static unsigned an_grid(u64 len, u32 batch) { return (unsigned)((len + AN_CHUNK 
 
 // R = NTT_N(r) of (p, g, n), built on first use on ctx->stream and kept until ronk_ctx_destroy (N words).
 static int anyntt_spectrum(ronk_ctx* ctx, u64 p, u64 g, u64 n, u32 log_N, const u64** out) {
-  const auto key = std::make_tuple((uint64_t)p, (uint64_t)g, (uint64_t)n);
-  auto it = ctx->anyntt_spec.find(key);
-  if (it == ctx->anyntt_spec.end()) {
-    const u64 N = (u64)1 << log_N;
-    u64* R = nullptr;
-    RONK_CUDA(ctx, cudaMalloc((void**)&R, N * sizeof(u64)));
-    int rc = [&] {
-      RONK_CUDA(ctx, cudaMemsetAsync(R, 0, N * sizeof(u64), ctx->stream));
-      RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
-        using F = std::decay_t<decltype(f)>;
-        return launch(ctx, "anyntt_chirp_table", anyntt_chirp_table_kernel<F>, an_grid(2 * n - 1, 1), AN_THREADS, 0, false, f,
-                      n, N, f.to_tw(h_powmod(g, (p - 1) / n, p)), R);
-      }));
-      return ntt_device(ctx, p, g, R, nullptr, log_N, 1, 0);
-    }();
-    if (rc != RONK_OK) {
-      cudaStreamSynchronize(ctx->stream);
-      cudaFree(R);
-      return rc;
-    }
-    it = ctx->anyntt_spec.emplace(key, R).first;
-  }
-  *out = it->second;
+  DevBuf<u64>& R = ctx->anyntt_spec[std::make_tuple((uint64_t)p, (uint64_t)g, (uint64_t)n)];  // empty until built
+  const u64 N = (u64)1 << log_N;
+  if (!R) RONK_TRY(build_table(ctx, &R, N, [&](u64* r) {
+    RONK_CUDA(ctx, cudaMemsetAsync(r, 0, N * sizeof(u64), ctx->stream));
+    RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
+      using F = std::decay_t<decltype(f)>;
+      return launch(ctx, "anyntt_chirp_table", anyntt_chirp_table_kernel<F>, an_grid(2 * n - 1, 1), AN_THREADS, 0, false, f, n,
+                    N, f.to_tw(h_powmod(g, (p - 1) / n, p)), r);
+    }));
+    return ntt_device(ctx, p, g, r, nullptr, log_N, 1, 0);
+  }));
+  *out = R.get();
   return RONK_OK;
 }
 

@@ -33,23 +33,16 @@ static int pairing_tables(ronk_ctx* ctx) {
   RONK_TRY(msm_coord_tables(ctx));
   uint16_t mu[PAIR_R];
   mu17_list(mu);
-  uint8_t* tab = nullptr;
-  RONK_CUDA(ctx, cudaMalloc((void**)&tab, kPairTabBytes + sizeof(mu)));
-  const u32* pttab = (const u32*)ctx->msm_coord + kTabWords;
-  int rc = RONK_OK;
-  cudaError_t e = cudaMemcpyAsync(tab + kPairTabBytes, mu, sizeof(mu), cudaMemcpyHostToDevice, ctx->stream);
-  if (e != cudaSuccess) rc = set_err(ctx, RONK_ECUDA, std::string("pairing table upload: ") + cudaGetErrorString(e));
-  if (rc == RONK_OK)
-    rc = launch(ctx, "pairing_table", pairing_table_kernel, (PAIR_TAB + PAIR_TAB_THREADS - 1) / PAIR_TAB_THREADS, PAIR_TAB_THREADS, 0,
-                false, pttab, (const uint16_t*)(tab + kPairTabBytes), tab);
-  if (rc == RONK_OK && (e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess)  // mu is on this stack frame
-    rc = set_err(ctx, RONK_ECUDA, std::string("pairing table build: ") + cudaGetErrorString(e));
-  if (rc != RONK_OK) {
-    cudaFree(tab);
-    return rc;
-  }
-  ctx->pairing_tab = tab;
-  return RONK_OK;
+  const u32* pttab = ctx->msm_coord.get() + kTabWords;
+  return build_table(ctx, &ctx->pairing_tab, kPairTabBytes + sizeof(mu), [&](uint8_t* tab) {
+    cudaError_t e = cudaMemcpyAsync(tab + kPairTabBytes, mu, sizeof(mu), cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) return set_err(ctx, RONK_ECUDA, std::string("pairing table upload: ") + cudaGetErrorString(e));
+    RONK_TRY(launch(ctx, "pairing_table", pairing_table_kernel, (PAIR_TAB + PAIR_TAB_THREADS - 1) / PAIR_TAB_THREADS,
+                    PAIR_TAB_THREADS, 0, false, pttab, (const uint16_t*)(tab + kPairTabBytes), tab));
+    if ((e = cudaStreamSynchronize(ctx->stream)) != cudaSuccess)  // mu is on this stack frame
+      return set_err(ctx, RONK_ECUDA, std::string("pairing table build: ") + cudaGetErrorString(e));
+    return RONK_OK;
+  });
 }
 
 __global__ void __launch_bounds__(KZG_CHECK_THREADS, 1)
@@ -144,8 +137,8 @@ int ronk_pairing_pluto_ext(ronk_ctx* ctx, const uint8_t* p, const uint8_t* q, si
   RONK_TRY(pairing_tables(ctx));
   volatile u32* flag = nullptr;
   RONK_TRY(clear_flag(ctx, &flag));
-  const u32* bintab = (const u32*)ctx->msm_coord;
-  const uint8_t* T = (const uint8_t*)ctx->pairing_tab;
+  const u32* bintab = ctx->msm_coord.get();
+  const uint8_t* T = ctx->pairing_tab.get();
   RONK_TRY(launch(ctx, "pairing", pairing_kernel, grid_for(ctx, n, PAIRING_THREADS), PAIRING_THREADS, 0, false, (const u32*)p,
                   (const u32*)q, n, bintab, T, (const uint16_t*)(T + kPairTabBytes), flag, out));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -180,7 +173,7 @@ int ronk_kzg_check_pluto_ext_batch(ronk_ctx* ctx, const uint8_t* commitments, co
   // a CTA is worth its 165 KB of tables once every thread sees ≥ 4 rows
   RONK_TRY(launch(ctx, "kzg_check", kzg_check_kernel, grid_for(ctx, n, KZG_CHECK_THREADS * 4, 1), KZG_CHECK_THREADS, kSmem, false,
                   (const u32*)commitments, (const u32*)proofs, points, values, n, (const u32*)g1_srs, (const u32*)g2_srs,
-                  (const u32*)ctx->msm_coord, (const uint8_t*)ctx->pairing_tab, flag, ok));
+                  (const u32*)ctx->msm_coord.get(), (const uint8_t*)ctx->pairing_tab.get(), flag, ok));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (ctx->h_flag[0])
     return set_err(ctx, RONK_EINVAL, "off-curve or non-canonical point, scalar >= 17, or a pairing argument the reference panics on");

@@ -382,7 +382,7 @@ static int divrem_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t da, c
     RONK_TRY(reset_flag(ctx));
     RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
       return launch(ctx, "poly_divrem", poly_divrem_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, a, (u32)da, b,
-                    (u32)db, q, r, ctx->d_flag);
+                    (u32)db, q, r, ctx->d_flag.get());
     }));
     int v = 0;
     RONK_TRY(read_flag(ctx, &v));  // synchronises the stream
@@ -463,7 +463,7 @@ static int divrem_batch_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t
   } else if (db) {
     RONK_TRY(reset_flag(ctx));
     RONK_TRY(launch(ctx, "divrem_top_scan", divrem_top_scan_kernel, grid_for(ctx, batch, 256), 256, 0, false, b, db, batch,
-                    ctx->d_flag));
+                    ctx->d_flag.get()));
     int zero = 0;
     RONK_TRY(read_flag(ctx, &zero));
     if (zero) path = DB_LITERAL;
@@ -504,7 +504,7 @@ static int divrem_batch_device(ronk_ctx* ctx, u64 p, u64 g, const u64* a, size_t
     RONK_TRY(reset_flag(ctx));
     RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
       return launch(ctx, "poly_divrem_rows", poly_divrem_rows_kernel<std::decay_t<decltype(f)>>, dim3(1, grid_rows(ctx, batch, 1)),
-                    256, 0, false, f, a, (u32)da, b, (u32)db, (u64)bs, batch, q, r, ctx->d_flag);
+                    256, 0, false, f, a, (u32)da, b, (u32)db, (u64)bs, batch, q, r, ctx->d_flag.get());
     }));
     int v = 0;
     RONK_TRY(read_flag(ctx, &v));  // synchronises the stream
@@ -677,7 +677,7 @@ static int interp_literal(ronk_ctx* ctx, u64 p, const u64* X, const u64* Y, size
     RONK_TRY(launch(ctx, "interp_master", interp_master_kernel<F>, 1, 1024, 0, false, f, X, (u32)k, m0, m1));
     const u64* M = (k & 1) ? m1 : m0;
     RONK_TRY(launch(ctx, "interp_nodes", interp_nodes_kernel<F>, dim3(blocks, grid_rows(ctx, rows, blocks)), 256, 0, false, f, M, X, Y,
-                    (u32)k, rows, partial, ctx->d_flag));
+                    (u32)k, rows, partial, ctx->d_flag.get()));
     return launch(ctx, "interp_sum", interp_sum_kernel<F>, dim3(blocks, grid_rows(ctx, rows, blocks)), 256, 0, false, f, partial, (u32)k,
                   nwarps, rows, out);
   }));
@@ -926,7 +926,7 @@ int ronk_poly_lagrange_eval_u64_host(ronk_ctx* ctx, uint64_t p, uint64_t g, cons
   RONK_TRY(reset_flag(ctx));
   RONK_TRY(with_field(ctx, p, 0, false, [&](const auto& f) {
     return launch(ctx, "lagrange_eval", lagrange_eval_kernel<std::decay_t<decltype(f)>>, 1, 256, 0, false, f, s[0].dev,
-                  s[1].dev, (u32)n, x, s[2].dev, ctx->d_flag);
+                  s[1].dev, (u32)n, x, s[2].dev, ctx->d_flag.get());
   }));
   int v = 0;
   RONK_TRY(read_flag(ctx, &v));

@@ -23,25 +23,43 @@ struct ProfRec {
   cudaEvent_t start, stop;
 };
 
+// Owns one cudaMalloc allocation of T and frees it when destroyed; move-only.  Its user has bound the device, as every
+// entry point does through DeviceGuard.
+template <class T>
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p_(o.p_) { o.p_ = nullptr; }
+  DevBuf& operator=(DevBuf&& o) noexcept { reset(); std::swap(p_, o.p_); return *this; }
+  ~DevBuf() { reset(); }
+  // frees what it held and allocates count elements; a failure is reported as RONK_CUDA does (no message for a null ctx)
+  int alloc(ronk_ctx* ctx, size_t count);
+  T* get() const { return p_; }
+  explicit operator bool() const { return p_ != nullptr; }
+  void reset() { if (p_) { cudaFree(p_); p_ = nullptr; } }
+
+ private:
+  T* p_ = nullptr;
+};
+
 struct NttPlan {
   u64 p = 0, g = 0;
   u32 log_n = 0;
   bool two_pass = false;
   u32 log_n1 = 0, log_n2 = 0;
-  u64* tw1 = nullptr;        // ω_{N1}^e (single pass: ω_n^e), twiddle form
-  u64* tw2 = nullptr;        // ω_{N2}^e == ω_n^(e·N1)
-  u64* tw1_2d[2] = {nullptr, nullptr};  // per-round 2-D tables of pass 1 / single (forward, inverse)
-  u64* tw2_2d[2] = {nullptr, nullptr};  // per-round 2-D tables of pass 2
-  u64* tw_lo = nullptr;      // ω_n^x, x < N1
-  u64* tw_hi_inv = nullptr;  // ω_n^(y·N1) · n^-1
+  DevBuf<u64> tw1;           // ω_{N1}^e (single pass: ω_n^e), twiddle form
+  DevBuf<u64> tw2;           // ω_{N2}^e == ω_n^(e·N1)
+  DevBuf<u64> tw1_2d[2];     // per-round 2-D tables of pass 1 / single (forward, inverse)
+  DevBuf<u64> tw2_2d[2];     // per-round 2-D tables of pass 2
+  DevBuf<u64> tw_lo;         // ω_n^x, x < N1
+  DevBuf<u64> tw_hi_inv;     // ω_n^(y·N1) · n^-1
   u64 scale_inv = 0;         // n^-1, twiddle form (single-pass inverse)
   // full inter-pass twiddle tables ω_n^(±j2·k1) [· n^-1] in the pass-1 workspace layout, per direction and
   // per log2(C2) of that layout (built on first use; n words each)
-  std::map<u32, u64*> tw_full[2];
+  std::map<u32, DevBuf<u64>> tw_full[2];
   // three-pass 2^24 transform (ntt3_kernel.cuh): ω_256^x and the 64 Ki-entry pass-2 table, per direction
-  u64* tw256[2] = {nullptr, nullptr};
-  u64* t2[2] = {nullptr, nullptr};
-  u64* t1[2] = {nullptr, nullptr};  // optional n-word pass-1 twiddle table (log n ≤ RONK_NTT3_T1)
+  DevBuf<u64> tw256[2], t2[2];
+  DevBuf<u64> t1[2];  // optional n-word pass-1 twiddle table (log n ≤ RONK_NTT3_T1)
 };
 
 // The context's per-call device scratch (Frame below): device blocks, of which blocks[0, used) hold the live regions,
@@ -106,6 +124,7 @@ struct ronk_tune {
 };
 
 struct ronk_ctx {
+  ~ronk_ctx();  // api.cu: what is not a DevBuf (events, the pipeline's streams, the scratch blocks, h_flag)
   int device = 0;
   ronk_tune tune;
   std::unordered_set<const void*> smem_attr_done;  // kernels whose >48 KiB dynamic-smem attribute is set on `device`
@@ -116,22 +135,22 @@ struct ronk_ctx {
   bool prof = false;
   std::vector<ronk::ProfRec> prof_log;
   std::map<std::tuple<uint64_t, uint64_t, uint32_t>, ronk::NttPlan> plans;
-  std::map<std::tuple<uint64_t, uint64_t, uint64_t>, uint64_t*> anyntt_spec;  // (p, g, n) → Bluestein spectrum, N words (ntt_any.cu)
+  std::map<std::tuple<uint64_t, uint64_t, uint64_t>, ronk::DevBuf<uint64_t>> anyntt_spec;  // (p, g, n) → Bluestein spectrum, N words (ntt_any.cu)
   ronk::Scratch scratch;  // every per-call device buffer: transform workspaces, operands, staged _host arguments
   // two-slot host pipeline (ronk_ntt_u64_host_submit / _wait)
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   static constexpr int kSlots = 3;
-  void* slot_buf[kSlots] = {};
+  ronk::DevBuf<uint64_t> slot_buf[kSlots];
   size_t slot_bytes[kSlots] = {};
   cudaEvent_t ev_h2d[kSlots] = {}, ev_compute[kSlots] = {}, ev_d2h[kSlots] = {};
   bool slot_pending[kSlots] = {};
   int cluster16_state = 0;   // ntt16c_kernel: 0 = not probed, 1 = usable, -1 = the device refuses 16-CTA clusters of its footprint
   void* dist = nullptr;      // ronk::DistState (dist.cu): communicator, peer mappings, staging — null until ronk_dist_init
-  void* msm_ytab = nullptr;  // uint16_t[20402]: y of the curve point in each histogram bin (msm.cu), built on first use
-  void* msm_done = nullptr;  // u32 completion counter of msm_hist_finish_kernel
-  void* msm_coord = nullptr; // msm_coord_kernel: bintab[20404] | pttab[10404] | counter, Σa, Σb (msm.cu), built on first use
-  void* pairing_tab = nullptr;  // uint8_t T[289²] of the Tate pairing on E[17], padded | μ17 list (pairing.cu), built on first use
-  int* d_flag = nullptr;  // device error flag
+  ronk::DevBuf<uint16_t> msm_ytab;  // [20402]: y of the curve point in each histogram bin (msm.cu), built on first use
+  ronk::DevBuf<uint32_t> msm_done;  // completion counter of msm_hist_finish_kernel + global histogram, built with msm_ytab
+  ronk::DevBuf<uint32_t> msm_coord; // msm_coord_kernel: bintab[20404] | pttab[10404] | counter, Σa, Σb (msm.cu), built on first use
+  ronk::DevBuf<uint8_t> pairing_tab;  // T[289²] of the Tate pairing on E[17], padded | μ17 list (pairing.cu), built on first use
+  ronk::DevBuf<int> d_flag;  // device error flag
   int* h_flag = nullptr;  // pinned host mirror: h_flag[0] = error flag, h_flag[1..31] = small results (msm.cu)
 };
 
@@ -155,6 +174,41 @@ inline int set_err(ronk_ctx* ctx, int code, const std::string& msg) {
     int _rc = (expr);           \
     if (_rc != RONK_OK) return _rc; \
   } while (0)
+
+template <class T>
+int DevBuf<T>::alloc(ronk_ctx* ctx, size_t count) {
+  reset();
+  T* p = nullptr;
+  RONK_CUDA(ctx, cudaMalloc((void**)&p, count * sizeof(T)));
+  p_ = p;
+  return RONK_OK;
+}
+
+// Tables a context or plan keeps once built on first use: build() allocates them into the caller's local DevBufs and
+// fills them on ctx->stream; the caller moves them into the context or plan only after build_tables returned RONK_OK.
+// On failure ctx->stream is synchronised, since queued work may still touch the locals, which then free themselves.
+template <class Build>
+inline int build_tables(ronk_ctx* ctx, Build&& build) {
+  const int rc = build();
+  if (rc != RONK_OK) cudaStreamSynchronize(ctx->stream);
+  return rc;
+}
+// The same for one table of count T: fill(ptr) fills it, and *slot takes it once filled.  optional: a table its user can
+// do without; where its allocation fails, CUDA's error is cleared, *slot stays empty (the next call tries again) and the
+// result is RONK_OK.
+template <class T, class Fill>
+inline int build_table(ronk_ctx* ctx, DevBuf<T>* slot, size_t count, Fill&& fill, bool optional = false) {
+  DevBuf<T> tab;
+  const int rc = tab.alloc(optional ? nullptr : ctx, count);
+  if (rc != RONK_OK) {
+    if (!optional) return rc;
+    cudaGetLastError();
+    return RONK_OK;
+  }
+  RONK_TRY(build_tables(ctx, [&] { return fill(tab.get()); }));
+  *slot = std::move(tab);
+  return RONK_OK;
+}
 
 // Binds the calling thread to the context's device for the duration of one C-ABI call and restores the
 // caller's device on exit (contexts for several GPUs may coexist in one process; the caller — torch, a
@@ -338,11 +392,11 @@ class Frame {
 // The device error flag that kernels raise with atomicExch: cleared before a launch, read back (synchronising the
 // stream) after it.
 inline int reset_flag(ronk_ctx* ctx) {
-  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag, 0, sizeof(int), ctx->stream));
+  RONK_CUDA(ctx, cudaMemsetAsync(ctx->d_flag.get(), 0, sizeof(int), ctx->stream));
   return RONK_OK;
 }
 inline int read_flag(ronk_ctx* ctx, int* v) {
-  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  RONK_CUDA(ctx, cudaMemcpyAsync(ctx->h_flag, ctx->d_flag.get(), sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   RONK_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   *v = *ctx->h_flag;
   return RONK_OK;
