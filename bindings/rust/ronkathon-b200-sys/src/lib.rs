@@ -132,6 +132,12 @@ extern "C" {
   /// `kzg::check` of n openings against one SRS: ok[r] = 1 when the row verifies, else 0.  Device pointers.
   pub fn ronk_kzg_check_pluto_ext_batch(ctx: *mut ronk_ctx, commitments: *const u8, proofs: *const u8, points: *const u8, values: *const u8, n: usize, g1_srs: *const u8, n_g1: usize, g2_srs: *const u8, n_g2: usize, ok: *mut u8) -> c_int;
   pub fn ronk_kzg_check_pluto_ext_batch_host(ctx: *mut ronk_ctx, commitments: *const u8, proofs: *const u8, points: *const u8, values: *const u8, n: usize, g1_srs: *const u8, n_g1: usize, g2_srs: *const u8, n_g2: usize, ok: *mut u8) -> c_int;
+  /// The reference's Poseidon permutation on `batch` states of `width` words, in place.  Device pointers.
+  pub fn ronk_poseidon_permute_u64(ctx: *mut ronk_ctx, p: u64, width: u32, alpha: u64, num_f: u32, num_p: u32, rc: *const u64, mds: *const u64, states: *mut u64, batch: usize) -> c_int;
+  pub fn ronk_poseidon_permute_u64_host(ctx: *mut ronk_ctx, p: u64, width: u32, alpha: u64, num_f: u32, num_p: u32, rc: *const u64, mds: *const u64, states: *mut u64, batch: usize) -> c_int;
+  /// One fresh Poseidon sponge per row: absorb `len` words, squeeze `n_out` words.  Device pointers.
+  pub fn ronk_poseidon_sponge_u64(ctx: *mut ronk_ctx, p: u64, width: u32, alpha: u64, num_f: u32, num_p: u32, rc: *const u64, mds: *const u64, rate: u32, input: *const u64, len: usize, batch: usize, out: *mut u64, n_out: usize) -> c_int;
+  pub fn ronk_poseidon_sponge_u64_host(ctx: *mut ronk_ctx, p: u64, width: u32, alpha: u64, num_f: u32, num_p: u32, rc: *const u64, mds: *const u64, rate: u32, input: *const u64, len: usize, batch: usize, out: *mut u64, n_out: usize) -> c_int;
   pub fn ronk_msm_pluto_ext_buckets(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, buckets: *mut u8) -> c_int;
   pub fn ronk_msm_combine_buckets_host(ctx: *mut ronk_ctx, buckets: *const u8, n_sets: usize, out: *mut u8) -> c_int;
 

@@ -556,6 +556,42 @@ int ronk_kzg_check_pluto_ext_batch(ronk_ctx *ctx, const uint8_t *commitments, co
 int ronk_kzg_check_pluto_ext_batch_host(ronk_ctx *ctx, const uint8_t *commitments, const uint8_t *proofs,
                                         const uint8_t *points, const uint8_t *values, size_t n,
                                         const uint8_t *g1_srs, size_t n_g1, const uint8_t *g2_srs, size_t n_g2, uint8_t *ok);
+/* ---- Poseidon (src/hashes/poseidon) ------------------------------------------------------------ */
+/* The reference's Poseidon permutation (poseidon/mod.rs:137-149) and sponge (sponge.rs:71-294) over F_p on batches of
+ * rows.  A configuration is (width T, alpha, num_f, num_p, rc, mds) as PoseidonConfig::new (mod.rs:39-56) takes it:
+ * rc holds R·T words with R = num_f + num_p, mds holds T² words row-major (mds[i·T + j] is mds[i][j]).  Round i adds
+ * rc[i·T ..], raises every element to alpha when i < num_f/2 or i ≥ num_p + num_f/2 and element 0 only otherwise
+ * (mod.rs:87-93), then multiplies by the MDS matrix, literally; x^0 = 1 for every x, as Field::pow gives.  Rows are
+ * contiguous and row-major.  All pointers of the device entries are DEVICE pointers.
+ * - ronk_poseidon_permute_u64: replaces each of the batch states (T words each) by its permutation.  Poseidon::hash is
+ *   this on the state zero-padded to T words, then word 1.
+ * - ronk_poseidon_sponge_u64: row y gets a fresh PoseidonSponge of this rate (capacity T − rate), absorbs
+ *   in[y·len, (y+1)·len), starts squeezing and squeezes n_out words into out[y·n_out ..].  Any split of the absorbed
+ *   words into absorb calls and of the squeezed count into squeeze calls gives these words.  len == 0 runs no
+ *   permutation before the first squeeze, as start_squeezing runs one only when absorb_index != 0.
+ * - Errors, in this order: (1) without reading a pointer: RONK_EINVAL for a null ctx, or a null pointer the call would
+ *   read or write (states when batch > 0; in when batch·len > 0; out when batch·n_out > 0; rc and mds when batch > 0
+ *   and R > 0); the modulus check every F_p entry makes (p = 2 is RONK_EUNSUPPORTED, a composite p RONK_EINVAL);
+ *   RONK_EINVAL for T < 2 (the reference's assert), and for the sponge rate == 0 or rate > T; RONK_EUNSUPPORTED for
+ *   T > 16, for R·T + T² above 6144 words of constants (48 KiB of shared memory: up to 368 rounds at T = 16), and for
+ *   batch·T, batch·len or batch·n_out above 2^40 words; (2) RONK_EINVAL when the output (states, out) overlaps rc, mds
+ *   (when R > 0) or, for the sponge, in.  On a refusal nothing has been enqueued or written.  batch == 0 does nothing,
+ *   and so does n_out == 0.  The words must be canonical residues (< p); the device entries do not check them, and
+ *   give unspecified words for others.
+ * - Launches: one whatever the batch, one thread per row (128-thread CTAs, at most 8 per SM, grid-stride).  Each CTA
+ *   holds the constants in shared memory.  Asynchronous on the context's stream.
+ * - The _host twins make every check of (1), then refuse a non-canonical word of rc, mds and the states or in with
+ *   RONK_EINVAL before they stage anything; they stage in and out and synchronise. */
+int ronk_poseidon_permute_u64(ronk_ctx *ctx, uint64_t p, uint32_t width, uint64_t alpha, uint32_t num_f, uint32_t num_p,
+                              const uint64_t *rc, const uint64_t *mds, uint64_t *states, size_t batch);
+int ronk_poseidon_permute_u64_host(ronk_ctx *ctx, uint64_t p, uint32_t width, uint64_t alpha, uint32_t num_f,
+                                   uint32_t num_p, const uint64_t *rc, const uint64_t *mds, uint64_t *states, size_t batch);
+int ronk_poseidon_sponge_u64(ronk_ctx *ctx, uint64_t p, uint32_t width, uint64_t alpha, uint32_t num_f, uint32_t num_p,
+                             const uint64_t *rc, const uint64_t *mds, uint32_t rate, const uint64_t *in, size_t len,
+                             size_t batch, uint64_t *out, size_t n_out);
+int ronk_poseidon_sponge_u64_host(ronk_ctx *ctx, uint64_t p, uint32_t width, uint64_t alpha, uint32_t num_f,
+                                  uint32_t num_p, const uint64_t *rc, const uint64_t *mds, uint32_t rate,
+                                  const uint64_t *in, size_t len, size_t batch, uint64_t *out, size_t n_out);
 /* Per-device partial MSM for the multi-GPU path: writes the 17 bucket sums (17×4 bytes, host)
  * so ranks can combine them; ronk_msm_combine_buckets folds world×17 buckets into one point. */
 int ronk_msm_pluto_ext_buckets(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t buckets[68]);

@@ -10,6 +10,7 @@ include/ronk_b200.h).  This package is the host-side mirror of the reference's s
     ops.*  — device-resident operator API on torch tensors (what bench.py times)
     dist.* — multi-GPU sharding (batch ranges, one-all-to-all distributed transform, MSM all-gather)
     codes.* — next rows: Reed–Solomon encode, Shamir-style multi-point evaluation
+    hashes.PoseidonConfig / Poseidon / PoseidonSponge — the reference's Poseidon over any prime field
 
 There is no CPU fallback: importing works anywhere, but creating a Context needs an H100.
 """
@@ -17,4 +18,4 @@ from ._lib import GOLDILOCKS, Context, RonkError, RonkPanic, default_context, se
 from .curve import AffinePoint, G1_GENERATOR, G2_GENERATOR  # noqa: F401
 from .field import GoldilocksField, PlutoBaseField, PlutoScalarField, PrimeField  # noqa: F401
 from .polynomial import Lagrange, Monomial, Polynomial  # noqa: F401
-from . import codes, dist, kzg, ops  # noqa: F401
+from . import codes, dist, hashes, kzg, ops  # noqa: F401

@@ -105,6 +105,10 @@ SIGNATURES = {
     "ronk_pairing_pluto_ext_host": (i32, [vp, vp, vp, sz, vp]),
     "ronk_kzg_check_pluto_ext_batch": (i32, [vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, vp]),
     "ronk_kzg_check_pluto_ext_batch_host": (i32, [vp, vp, vp, vp, vp, sz, vp, sz, vp, sz, vp]),
+    "ronk_poseidon_permute_u64": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, vp, sz]),
+    "ronk_poseidon_permute_u64_host": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, vp, sz]),
+    "ronk_poseidon_sponge_u64": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, u32, vp, sz, sz, vp, sz]),
+    "ronk_poseidon_sponge_u64_host": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, u32, vp, sz, sz, vp, sz]),
     "ronk_msm_pluto_ext_buckets": (i32, [vp, vp, sz, vp, sz, vp]),
     "ronk_msm_combine_buckets_host": (i32, [vp, vp, sz, vp]),
     "ronk_splitmix_fill_u64": (i32, [vp, u64, u64, vp, sz]),

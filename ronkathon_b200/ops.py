@@ -333,6 +333,45 @@ def kzg_check(ctx: Context, C, Pi, z, v, g1_srs, g2_srs):
     return ok
 
 
+def poseidon_permute_(ctx: Context, states, cfg, p: int | None = None):
+    """The reference's Poseidon permutation (hashes/poseidon/mod.rs:137-149) of every row of states, a contiguous
+    [batch, width] device tensor, in place, in one launch.  cfg: a hashes.PoseidonConfig; p defaults to its field's
+    modulus (Goldilocks for plain-int constants).  Asynchronous on the context's stream."""
+    _check_u64(states)
+    p = cfg.modulus(p)
+    assert states.dim() == 2 and states.shape[1] == cfg.width, "states is a [batch, width] tensor"
+    ctx.call("ronk_poseidon_permute_u64", *cfg.args(ctx, p), _lib._ptr(states), states.shape[0])
+    return states
+
+
+def poseidon_hash(ctx: Context, rows, cfg, p: int | None = None):
+    """Poseidon::hash (mod.rs:137-149) of every row of rows ([batch, k] device tensor, k ≤ width): zero-padded to width,
+    permuted, word 1.  A new [batch] tensor.  The padding and the column are torch operations on the current stream,
+    which the context is expected to share, as for every tensor this module allocates."""
+    import torch
+    _check_u64(rows)
+    assert rows.dim() == 2, "rows is a [batch, k] tensor"
+    if rows.shape[1] > cfg.width:
+        raise _lib.RonkPanic(_lib.EINVAL, "state longer than the hash width (poseidon/mod.rs:138 underflows)")
+    states = torch.zeros((rows.shape[0], cfg.width), dtype=torch.int64, device=rows.device)
+    states[:, :rows.shape[1]] = rows
+    poseidon_permute_(ctx, states, cfg, p)
+    return states[:, 1].contiguous()
+
+
+def poseidon_sponge(ctx: Context, rows, n_out: int, rate: int, cfg, p: int | None = None):
+    """One fresh PoseidonSponge (hashes/poseidon/sponge.rs) per row of rows ([batch, len] device tensor): absorb the row,
+    start squeezing, squeeze n_out words.  A new [batch, n_out] tensor; asynchronous on the context's stream."""
+    import torch
+    _check_u64(rows)
+    assert rows.dim() == 2, "rows is a [batch, len] tensor"
+    p = cfg.modulus(p)
+    out = torch.empty((rows.shape[0], n_out), dtype=torch.int64, device=rows.device)
+    ctx.call("ronk_poseidon_sponge_u64", *cfg.args(ctx, p), rate, _lib._ptr(rows), rows.shape[1], rows.shape[0],
+             _lib._ptr(out), n_out)
+    return out
+
+
 def msm_buckets(ctx: Context, points, scalars) -> bytes:
     out = np.empty(68, dtype=np.uint8)
     ctx.call("ronk_msm_pluto_ext_buckets", _lib._ptr(points), points.numel() // 4, _lib._ptr(scalars),

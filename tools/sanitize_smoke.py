@@ -33,5 +33,12 @@ g1, g2 = kzg.setup()
 cm, pf = kzg.commit([3, 2, 1], g1), kzg.open_([3, 2, 1], 5, g1)
 ok &= kzg.check_batch([cm] * 3, [pf] * 3, [5] * 3, [4, 10, 4], g1, g2) == [True, False, True]
 ok &= curve.pairing(curve.AffinePoint(bytes([9, 37, 19, 93])), curve.AffinePoint(bytes([63, 0, 0, 35]))) == (26, 97)
+import poseidon_oracle as po
+from ronkathon_b200.hashes import PoseidonConfig
+orc = po.Config(GL, 5, 7, 3, 4, oracle.splitmix(GL, 4, 7 * 5).tolist(), oracle.splitmix(GL, 5, 25).reshape(5, 5).tolist())
+pcfg = PoseidonConfig(5, 7, 3, 4, orc.rc.tolist(), orc.mds.reshape(5, 5).tolist())
+st = oracle.splitmix(GL, 6, 300 * 5).reshape(300, 5)
+ok &= np.array_equal(host(ops.poseidon_permute_(c, dev(st).view(300, 5), pcfg)).reshape(300, 5), po.permute(orc, st))
+ok &= np.array_equal(host(ops.poseidon_sponge(c, dev(st).view(300, 5), 7, 3, pcfg)).reshape(300, 7), po.sponge_rows(orc, 3, st, 7))
 print("sanitize_smoke", "OK" if ok else "MISMATCH")
 sys.exit(0 if ok else 1)
