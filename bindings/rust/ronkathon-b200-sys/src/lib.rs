@@ -138,6 +138,18 @@ extern "C" {
   /// One fresh Poseidon sponge per row: absorb `len` words, squeeze `n_out` words.  Device pointers.
   pub fn ronk_poseidon_sponge_u64(ctx: *mut ronk_ctx, p: u64, width: u32, alpha: u64, num_f: u32, num_p: u32, rc: *const u64, mds: *const u64, rate: u32, input: *const u64, len: usize, batch: usize, out: *mut u64, n_out: usize) -> c_int;
   pub fn ronk_poseidon_sponge_u64_host(ctx: *mut ronk_ctx, p: u64, width: u32, alpha: u64, num_f: u32, num_p: u32, rc: *const u64, mds: *const u64, rate: u32, input: *const u64, len: usize, batch: usize, out: *mut u64, n_out: usize) -> c_int;
+  /// SHA-256 of n messages data[offsets[i], offsets[i+1]): out[32·i ..].  Device pointers.
+  pub fn ronk_sha256(ctx: *mut ronk_ctx, data: *const u8, data_len: u64, offsets: *const u64, n: usize, out: *mut u8) -> c_int;
+  pub fn ronk_sha256_host(ctx: *mut ronk_ctx, data: *const u8, data_len: u64, offsets: *const u64, n: usize, out: *mut u8) -> c_int;
+  /// Every level of the SHA-256 Merkle tree of n messages, leaf level first.  Device pointers.
+  pub fn ronk_merkle_build_sha256(ctx: *mut ronk_ctx, data: *const u8, data_len: u64, offsets: *const u64, n: usize, nodes: *mut u8) -> c_int;
+  pub fn ronk_merkle_build_sha256_host(ctx: *mut ronk_ctx, data: *const u8, data_len: u64, offsets: *const u64, n: usize, nodes: *mut u8) -> c_int;
+  /// `get_proof` of m leaf indices: L siblings and sides (0 = Left, 1 = Right) each.  Device pointers.
+  pub fn ronk_merkle_proofs_sha256(ctx: *mut ronk_ctx, nodes: *const u8, n: usize, indices: *const u64, m: usize, siblings: *mut u8, sides: *mut u8) -> c_int;
+  pub fn ronk_merkle_proofs_sha256_host(ctx: *mut ronk_ctx, nodes: *const u8, n: usize, indices: *const u64, m: usize, siblings: *mut u8, sides: *mut u8) -> c_int;
+  /// `prove` of m messages with depth-step proofs against one root: ok[j] = 1 or 0.  Device pointers.
+  pub fn ronk_merkle_verify_sha256(ctx: *mut ronk_ctx, root: *const u8, data: *const u8, data_len: u64, offsets: *const u64, m: usize, siblings: *const u8, sides: *const u8, depth: u32, ok: *mut u8) -> c_int;
+  pub fn ronk_merkle_verify_sha256_host(ctx: *mut ronk_ctx, root: *const u8, data: *const u8, data_len: u64, offsets: *const u64, m: usize, siblings: *const u8, sides: *const u8, depth: u32, ok: *mut u8) -> c_int;
   pub fn ronk_msm_pluto_ext_buckets(ctx: *mut ronk_ctx, points: *const u8, n_points: usize, scalars: *const u8, n_scalars: usize, buckets: *mut u8) -> c_int;
   pub fn ronk_msm_combine_buckets_host(ctx: *mut ronk_ctx, buckets: *const u8, n_sets: usize, out: *mut u8) -> c_int;
 

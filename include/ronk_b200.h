@@ -592,6 +592,55 @@ int ronk_poseidon_sponge_u64(ronk_ctx *ctx, uint64_t p, uint32_t width, uint64_t
 int ronk_poseidon_sponge_u64_host(ronk_ctx *ctx, uint64_t p, uint32_t width, uint64_t alpha, uint32_t num_f,
                                   uint32_t num_p, const uint64_t *rc, const uint64_t *mds, uint32_t rate,
                                   const uint64_t *in, size_t len, size_t batch, uint64_t *out, size_t n_out);
+/* ---- SHA-256 and Merkle trees (src/hashes/sha.rs, src/tree/merkle.rs) ------------------------------------------ */
+/* The reference's Sha256::digest (sha.rs:88-201: standard SHA-256) on batches of byte strings, and its MerkleTree
+ * (merkle.rs:31-98) built, opened and verified on the device.  A digest is 32 bytes, h0 … h7 each big-endian.  A batch
+ * of n messages is data[offsets[i], offsets[i+1]) for i < n: offsets holds n + 1 uint64_t, non-decreasing, with
+ * offsets[n] ≤ data_len; any start alignment.  All pointers of the device entries are DEVICE pointers.
+ * - Tree layout: level l (0 = the leaves' digests) holds s_l = ⌈n / 2^l⌉ nodes, l = 0 … L with L = ⌈log2 n⌉ for n ≥ 2
+ *   and L = 0 for n = 1; level l + 1 node i is digest(level_l[2i] ‖ level_l[2i + 1]), the last node of an odd level
+ *   paired with itself.  `nodes` holds the levels leaf level first, each contiguous: level l starts at node
+ *   off_l = Σ_{k<l} s_k (byte 32·off_l), the root is node off_L, and the buffer is (off_L + 1)·32 bytes.  The reference
+ *   stores the same levels root first (MerkleTree::hashes).
+ * - ronk_sha256: out[32·i ..] = digest(message i).  One launch.
+ * - ronk_merkle_build_sha256: every level of the tree of the n messages into nodes.  n == 0 does nothing (the
+ *   reference's tree of no leaves has no root).  1 + ⌈max(L − 9, 0) / 9⌉ launches: each CTA reduces 512 nodes through
+ *   up to 9 levels in shared memory.
+ * - ronk_merkle_proofs_sha256: get_proof (merkle.rs:66-81) of each of the m leaf indices against the tree of n leaves
+ *   in nodes (as built above): for l < L, siblings[(j·L + l)·32 ..] = node (indices[j] >> l) ^ 1 of level l and
+ *   sides[j·L + l] = 1 (Right) when indices[j] >> l is even, else 0 (Left).  An index at which that sibling lies past
+ *   its level is where the reference panics (e.g. n = 5: indices 4 and 5; n = 3: index 3 is accepted).  n ≤ 1 gives
+ *   L = 0 and empty proofs.  One launch when m·L > 0.
+ * - ronk_merkle_verify_sha256: ok[j] = 1 when prove (merkle.rs:84-98) holds for message j of the m messages with the
+ *   depth steps siblings[(j·depth + l)·32 ..], sides[j·depth + l] (0 = Left: digest(sibling ‖ h), 1 = Right:
+ *   digest(h ‖ sibling)) against the 32-byte root, else 0.  depth may be 0.  One launch.
+ * - Errors, in this order: (1) without reading memory: RONK_EINVAL for a null ctx or a null pointer the call would use
+ *   (data may be null when data_len == 0; offsets and the output when n or m is 0; the proofs' pointers when m·L == 0;
+ *   siblings and sides when depth == 0), and for offsets or indices not 8-byte aligned (device entries);
+ *   RONK_EUNSUPPORTED for n or m ≥ 2^32, data_len > 2^40 or depth > 32; (2) RONK_EINVAL for an output that overlaps an
+ *   input (or, for the proofs, the other output); nothing is enqueued or written before this point, and no scratch is
+ *   taken; (3) the call runs, synchronises once, and returns RONK_EINVAL if the device saw offsets that decrease or pass
+ *   data_len, a proof index at which get_proof panics, or a side byte other than 0 or 1.  Output contents are then
+ *   unspecified.  No kernel reads data outside [offsets[0], offsets[n]) or nodes outside the tree, whatever the input.
+ * - The _host twins take host pointers, make the checks of (1), refuse bad offsets and side bytes on the host before
+ *   they stage anything, then stage and synchronise. */
+int ronk_sha256(ronk_ctx *ctx, const uint8_t *data, uint64_t data_len, const uint64_t *offsets, size_t n, uint8_t *out);
+int ronk_sha256_host(ronk_ctx *ctx, const uint8_t *data, uint64_t data_len, const uint64_t *offsets, size_t n,
+                     uint8_t *out);
+int ronk_merkle_build_sha256(ronk_ctx *ctx, const uint8_t *data, uint64_t data_len, const uint64_t *offsets, size_t n,
+                             uint8_t *nodes);
+int ronk_merkle_build_sha256_host(ronk_ctx *ctx, const uint8_t *data, uint64_t data_len, const uint64_t *offsets,
+                                  size_t n, uint8_t *nodes);
+int ronk_merkle_proofs_sha256(ronk_ctx *ctx, const uint8_t *nodes, size_t n, const uint64_t *indices, size_t m,
+                              uint8_t *siblings, uint8_t *sides);
+int ronk_merkle_proofs_sha256_host(ronk_ctx *ctx, const uint8_t *nodes, size_t n, const uint64_t *indices, size_t m,
+                                   uint8_t *siblings, uint8_t *sides);
+int ronk_merkle_verify_sha256(ronk_ctx *ctx, const uint8_t *root, const uint8_t *data, uint64_t data_len,
+                              const uint64_t *offsets, size_t m, const uint8_t *siblings, const uint8_t *sides,
+                              uint32_t depth, uint8_t *ok);
+int ronk_merkle_verify_sha256_host(ronk_ctx *ctx, const uint8_t *root, const uint8_t *data, uint64_t data_len,
+                                   const uint64_t *offsets, size_t m, const uint8_t *siblings, const uint8_t *sides,
+                                   uint32_t depth, uint8_t *ok);
 /* Per-device partial MSM for the multi-GPU path: writes the 17 bucket sums (17×4 bytes, host)
  * so ranks can combine them; ronk_msm_combine_buckets folds world×17 buckets into one point. */
 int ronk_msm_pluto_ext_buckets(ronk_ctx *ctx, const uint8_t *points, size_t n_points, const uint8_t *scalars, size_t n_scalars, uint8_t buckets[68]);

@@ -11,6 +11,7 @@ include/ronk_b200.h).  This package is the host-side mirror of the reference's s
     dist.* — multi-GPU sharding (batch ranges, one-all-to-all distributed transform, MSM all-gather)
     codes.* — next rows: Reed–Solomon encode, Shamir-style multi-point evaluation
     hashes.PoseidonConfig / Poseidon / PoseidonSponge — the reference's Poseidon over any prime field
+    hashes.Sha256, tree.MerkleTree — the reference's SHA-256 and its Merkle tree
 
 There is no CPU fallback: importing works anywhere, but creating a Context needs an H100.
 """
@@ -18,4 +19,4 @@ from ._lib import GOLDILOCKS, Context, RonkError, RonkPanic, default_context, se
 from .curve import AffinePoint, G1_GENERATOR, G2_GENERATOR  # noqa: F401
 from .field import GoldilocksField, PlutoBaseField, PlutoScalarField, PrimeField  # noqa: F401
 from .polynomial import Lagrange, Monomial, Polynomial  # noqa: F401
-from . import codes, dist, hashes, kzg, ops  # noqa: F401
+from . import codes, dist, hashes, kzg, ops, tree  # noqa: F401

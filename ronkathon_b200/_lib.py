@@ -109,6 +109,14 @@ SIGNATURES = {
     "ronk_poseidon_permute_u64_host": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, vp, sz]),
     "ronk_poseidon_sponge_u64": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, u32, vp, sz, sz, vp, sz]),
     "ronk_poseidon_sponge_u64_host": (i32, [vp, u64, u32, u64, u32, u32, vp, vp, u32, vp, sz, sz, vp, sz]),
+    "ronk_sha256": (i32, [vp, vp, u64, vp, sz, vp]),
+    "ronk_sha256_host": (i32, [vp, vp, u64, vp, sz, vp]),
+    "ronk_merkle_build_sha256": (i32, [vp, vp, u64, vp, sz, vp]),
+    "ronk_merkle_build_sha256_host": (i32, [vp, vp, u64, vp, sz, vp]),
+    "ronk_merkle_proofs_sha256": (i32, [vp, vp, sz, vp, sz, vp, vp]),
+    "ronk_merkle_proofs_sha256_host": (i32, [vp, vp, sz, vp, sz, vp, vp]),
+    "ronk_merkle_verify_sha256": (i32, [vp, vp, vp, u64, vp, sz, vp, vp, u32, vp]),
+    "ronk_merkle_verify_sha256_host": (i32, [vp, vp, vp, u64, vp, sz, vp, vp, u32, vp]),
     "ronk_msm_pluto_ext_buckets": (i32, [vp, vp, sz, vp, sz, vp]),
     "ronk_msm_combine_buckets_host": (i32, [vp, vp, sz, vp]),
     "ronk_splitmix_fill_u64": (i32, [vp, u64, u64, vp, sz]),

@@ -114,15 +114,6 @@ static int check_args(ronk_ctx* ctx, const uint8_t* commitments, const uint8_t* 
   return RONK_OK;
 }
 
-// The mapped pinned error flag, cleared: its device address for the kernel.
-static int clear_flag(ronk_ctx* ctx, volatile u32** dev) {
-  ((volatile u32*)ctx->h_flag)[0] = 0u;
-  u32* d = nullptr;
-  RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&d, (void*)ctx->h_flag, 0));
-  *dev = d;
-  return RONK_OK;
-}
-
 }  // namespace ronk
 
 using namespace ronk;

@@ -402,6 +402,16 @@ inline int read_flag(ronk_ctx* ctx, int* v) {
   return RONK_OK;
 }
 
+// The mapped pinned error flag, cleared: its device address for a kernel that raises it with a plain store.  The
+// caller synchronises ctx->stream before it reads h_flag[0] (pairing.cu, sha256.cu).
+inline int clear_flag(ronk_ctx* ctx, volatile u32** dev) {
+  ((volatile u32*)ctx->h_flag)[0] = 0u;
+  u32* d = nullptr;
+  RONK_CUDA(ctx, cudaHostGetDevicePointer((void**)&d, (void*)ctx->h_flag, 0));
+  *dev = d;
+  return RONK_OK;
+}
+
 // One region of a _host call's arguments: `bytes` uploaded from `in` before the call when `in` is set, downloaded to
 // `out` after a successful call when `out` is set, scratch when neither is.
 struct Staged {

@@ -1,10 +1,11 @@
 """Host-side mirror of ronkathon's `hashes::poseidon` (src/hashes/poseidon/{mod,sponge}.rs): `PoseidonConfig`,
-`Poseidon::hash` and `PoseidonSponge` with its Init → Absorbing → Squeezing typestate, over any prime field.
+`Poseidon::hash` and `PoseidonSponge` with its Init → Absorbing → Squeezing typestate, over any prime field; and of
+`hashes::sha::Sha256` (src/hashes/sha.rs), whose digests run in libronk_b200.so (`ronk_sha256`).
 
 Every permutation runs in libronk_b200.so (`ronk_poseidon_permute_u64`).  The single-object classes keep their state on
 the host and permute a batch of one state per call, which is literal and slow; `ops.poseidon_permute_`,
-`ops.poseidon_hash` and `ops.poseidon_sponge` are the batched device paths.  The other hashes of `src/hashes` (SHA-2,
-SHA-3, GHASH) are not mirrored.
+`ops.poseidon_hash` and `ops.poseidon_sponge` are the batched device paths, as `ops.sha256` is for SHA-256.  The other
+hashes of `src/hashes` (SHA-512, SHA-3, GHASH) are not mirrored.
 """
 from __future__ import annotations
 
@@ -217,3 +218,16 @@ class PoseidonSponge:
             if self.squeeze_index == self.rate:
                 self.permute()
                 self.squeeze_index = 0
+
+
+class Sha256:
+    """Sha256 (sha.rs:203-232): `Sha256().digest(input)` is the 32-byte SHA-256 of the bytes, computed on the device as a
+    batch of one message (`ronk_sha256_host` on the default context)."""
+
+    def digest(self, data) -> bytes:
+        m = np.frombuffer(bytes(data), dtype=np.uint8)
+        offsets = np.array([0, m.size], dtype=np.uint64)
+        out = np.empty(32, dtype=np.uint8)
+        _lib.default_context().call("ronk_sha256_host", _lib._ptr(m) if m.size else None, m.size, _lib._ptr(offsets), 1,
+                                    _lib._ptr(out))
+        return out.tobytes()

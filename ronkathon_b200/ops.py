@@ -372,6 +372,88 @@ def poseidon_sponge(ctx: Context, rows, n_out: int, rate: int, cfg, p: int | Non
     return out
 
 
+def _check_u8(t):
+    import torch
+    assert t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous(), "need a contiguous CUDA uint8 tensor"
+
+
+def merkle_levels(n: int):
+    """(sizes, offsets) of the levels of a SHA-256 Merkle tree of n ≥ 1 leaves, leaf level first, as the node buffer of
+    merkle_build lays them out: level l holds ⌈n / 2^l⌉ nodes from node offsets[l] on, l = 0 … L, L = ⌈log2 n⌉."""
+    sizes = [n]
+    while sizes[-1] > 1:
+        sizes.append((sizes[-1] + 1) // 2)
+    offsets = [sum(sizes[:l]) for l in range(len(sizes))]
+    return sizes, offsets
+
+
+def _messages(data, offsets):
+    _check_u8(data)
+    _check_u64(offsets)
+    assert offsets.dim() == 1 and offsets.numel() >= 1, "offsets holds n + 1 entries"
+    return offsets.numel() - 1
+
+
+def sha256(ctx: Context, data, offsets):
+    """SHA-256 (hashes/sha.rs:88-201) of each message data[offsets[i]:offsets[i+1]] of a uint8 device tensor; offsets is
+    an int64 device tensor of n + 1 entries.  A new [n, 32] uint8 tensor; one launch, then one synchronisation to check
+    the offsets (RonkPanic when they decrease or pass the data)."""
+    import torch
+    n = _messages(data, offsets)
+    out = torch.empty((n, 32), dtype=torch.uint8, device=data.device)
+    ctx.call("ronk_sha256", _lib._ptr(data) if data.numel() else None, data.numel(), _lib._ptr(offsets), n, _lib._ptr(out))
+    return out
+
+
+def merkle_build(ctx: Context, data, offsets):
+    """MerkleTree::new (tree/merkle.rs:31-60) over the messages of data and offsets (as sha256 takes them): (nodes, level
+    offsets).  nodes is a new [Σ sizes, 32] uint8 tensor holding every level, leaf level first; level l starts at row
+    level_offsets[l], and the root is the last row.  n = 0 gives an empty buffer and no levels."""
+    import torch
+    n = _messages(data, offsets)
+    if n == 0:
+        return torch.empty((0, 32), dtype=torch.uint8, device=data.device), []
+    sizes, level_offsets = merkle_levels(n)
+    nodes = torch.empty((sum(sizes), 32), dtype=torch.uint8, device=data.device)
+    ctx.call("ronk_merkle_build_sha256", _lib._ptr(data) if data.numel() else None, data.numel(), _lib._ptr(offsets), n,
+             _lib._ptr(nodes))
+    return nodes, level_offsets
+
+
+def merkle_proofs(ctx: Context, nodes, n: int, indices):
+    """get_proof (merkle.rs:66-81) of each leaf index (int64 device tensor [m]) against the tree of n leaves that
+    merkle_build wrote into nodes: (siblings [m, L, 32] uint8, sides [m, L] uint8, 0 = Left and 1 = Right).  An index at
+    which the reference panics raises RonkPanic."""
+    import torch
+    _check_u8(nodes)
+    _check_u64(indices)
+    depth = len(merkle_levels(n)[0]) - 1 if n else 0
+    m = indices.numel()
+    sib = torch.empty((m, depth, 32), dtype=torch.uint8, device=nodes.device)
+    sides = torch.empty((m, depth), dtype=torch.uint8, device=nodes.device)
+    ctx.call("ronk_merkle_proofs_sha256", _lib._ptr(nodes), n, _lib._ptr(indices), m, _lib._ptr(sib), _lib._ptr(sides))
+    return sib, sides
+
+
+def merkle_verify(ctx: Context, root, data, offsets, siblings, sides):
+    """prove (merkle.rs:84-98) of each message of data and offsets with its proof (siblings [m, depth, 32], sides
+    [m, depth] uint8 device tensors) against root (32-byte uint8 device tensor): a new [m] bool tensor."""
+    import torch
+    m = _messages(data, offsets)
+    _check_u8(root)
+    _check_u8(siblings)
+    _check_u8(sides)
+    assert root.numel() == 32, "root is 32 bytes"
+    assert sides.dim() == 2 and sides.shape[0] == m and siblings.shape == (m, sides.shape[1], 32), \
+        "siblings [m, depth, 32] and sides [m, depth]"
+    depth = sides.shape[1]
+    ok = torch.empty(m, dtype=torch.uint8, device=data.device)
+    ctx.call("ronk_merkle_verify_sha256", _lib._ptr(root), _lib._ptr(data) if data.numel() else None, data.numel(),
+             _lib._ptr(offsets), m, _lib._ptr(siblings) if siblings.numel() else None,
+             _lib._ptr(sides) if sides.numel() else None, depth, _lib._ptr(ok))
+    return ok.bool()
+
+
 def msm_buckets(ctx: Context, points, scalars) -> bytes:
     out = np.empty(68, dtype=np.uint8)
     ctx.call("ronk_msm_pluto_ext_buckets", _lib._ptr(points), points.numel() // 4, _lib._ptr(scalars),

@@ -40,5 +40,21 @@ pcfg = PoseidonConfig(5, 7, 3, 4, orc.rc.tolist(), orc.mds.reshape(5, 5).tolist(
 st = oracle.splitmix(GL, 6, 300 * 5).reshape(300, 5)
 ok &= np.array_equal(host(ops.poseidon_permute_(c, dev(st).view(300, 5), pcfg)).reshape(300, 5), po.permute(orc, st))
 ok &= np.array_equal(host(ops.poseidon_sponge(c, dev(st).view(300, 5), 7, 3, pcfg)).reshape(300, 7), po.sponge_rows(orc, 3, st, 7))
+import hashlib
+import merkle_oracle as mo
+leaves = [bytes(range(i % 5, i % 5 + i % 45)) for i in range(1100)]   # ragged, misaligned; two build launches
+lo = np.concatenate([[0], np.cumsum([len(x) for x in leaves])]).astype(np.uint64)
+ld = torch.frombuffer(bytearray(b"".join(leaves)), dtype=torch.uint8).cuda()
+dig = ops.sha256(c, ld, dev(lo)).cpu().numpy()
+ok &= all(dig[i].tobytes() == hashlib.sha256(leaves[i]).digest() for i in range(1100))
+nodes, _ = ops.merkle_build(c, ld, dev(lo))
+mt = mo.Tree(leaves)
+ok &= nodes.cpu().numpy().tobytes() == mt.nodes()
+picks = list(range(0, 1024, 9))
+sib, sides = ops.merkle_proofs(c, nodes, 1100, dev(np.array(picks, np.uint64)))
+items = [leaves[i] for i in picks]
+io = np.concatenate([[0], np.cumsum([len(x) for x in items])]).astype(np.uint64)
+ok &= bool(ops.merkle_verify(c, nodes[-1].contiguous(), torch.frombuffer(bytearray(b"".join(items)), dtype=torch.uint8).cuda(),
+                             dev(io), sib, sides).all())
 print("sanitize_smoke", "OK" if ok else "MISMATCH")
 sys.exit(0 if ok else 1)
